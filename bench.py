@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """SPG step benchmark (BASELINE.json: "SPG train-step edges+points/sec ...; ECC scatter HBM %peak").
 
-    python bench.py --gpus N --steps K --warmup W                 # this repo's sm_100a path, configs[1]
-    python bench.py --impl reference --steps K --warmup W         # the reference's own CPU modules
+    python bench.py --gpus N --steps K --warmup W                 # this repo's sm_90a path, configs[1]
+    python bench.py --impl reference --steps K --warmup W         # the CPU port of the reference's path
+    python bench.py ... --dump-outputs DIR                        # also write the last timed step's outputs
     python bench.py --workload room_fwd|sema3d_eval|vkitti_train|sweep_vv|sweep_mat [--nodes N]
 
 Default workload (the headline line): one full training step of configs[1] ("S3DIS Area-5 fold
@@ -20,11 +21,13 @@ Timing: every step is bracketed by CUDA events on the launching stream; an L2 fl
 memset) runs between steps outside the brackets; the reported time is the max over ranks of the
 summed step times, after a barrier + synchronize on both sides of the K steps.
 
-Reference arm: baseline/_ref/ holds a verbatim copy of the reference's learning/{pointnet,graphnet,
-modules}.py and learning/ecc/* (baseline/install_ref.py, run by __graft_entry__.build() where
-/root/reference exists; git-ignored, shipped with the snapshot).  `--impl reference` drives those
-modules through their own API on the host CPU (baseline/ref_arm.py); `cpu_baseline.kind` is
-"reference" then, "port" (oracle/nets_ref) only if the copy is missing.
+Reference arm: `--impl reference` and `cpu_baseline` time the oracle's port of the reference's CPU
+path (oracle/nets_ref, per-node ECC loops as in learning/ecc/GraphConvModule.py) on the host cores;
+`cpu_baseline.kind` is "port".
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (loss and logits of a
+training step, logits of an inference step) as DIR/<name>.npy in float32.  Model and batches are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -62,6 +65,8 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer pass (profiling runs)")
     ap.add_argument("--trace-gemm", action="store_true", help="per-shape timing of the SIMT GEMM calls (stderr)")
     ap.add_argument("--no-graph", action="store_true", help="time eager launches only (no CUDA-graph replay)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -72,7 +77,8 @@ def peaks():
         return dict(hbm=float(d["hbm_gbs"]), bf16=float(d["bf16_tflops"]),
                     bf16_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s; ceilings, not measurements
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, source="H100 SXM data sheet")
 
 
 def workload_counts(batch):
@@ -188,64 +194,37 @@ def host_info():
 
 
 class CpuArm(object):
-    """The reference's CPU path for one workload: the reference's OWN modules when baseline/_ref is
-    installed (kind "reference": baseline/ref_arm.py), else the oracle port (kind "port")."""
+    """The reference's CPU path for one workload, as the oracle ports it (kind "port")."""
 
     def __init__(self, w, sd_ecc=None, sd_ptn=None):
-        from baseline import ref_arm
         self.w, self.margs = w, w["margs"]
-        self.kind = "reference" if ref_arm.available() else "port"
+        self.kind = "port"
         self.sd = (sd_ecc, sd_ptn)
         self._make()
 
     def _make(self):
+        from oracle import nets_ref
+        from superpoint_graph_b200 import workloads
+        from superpoint_graph_b200.trainer import create_model
         sd_ecc, sd_ptn = self.sd
-        if self.kind == "reference":
-            from baseline import ref_arm
-            self.impl = ref_arm.ReferenceStep(self.margs, seed=1)
-            if sd_ecc is not None:
-                self.impl.load(sd_ecc, sd_ptn)
-        else:
-            from oracle import nets_ref
-            from superpoint_graph_b200 import workloads
-            from superpoint_graph_b200.trainer import create_model
-            if sd_ecc is None:
-                torch.manual_seed(1)
-                model = create_model(self.margs)
-                sd_ecc, sd_ptn = model.ecc.state_dict(), model.ptn.state_dict()
-            self.pcfg, self.mcfg = workloads.oracle_cfg(self.margs)
-            self.impl = nets_ref.RefTrainer(sd_ptn, sd_ecc, self.pcfg, self.mcfg, lr=self.margs.lr,
-                                            grad_clip=self.margs.grad_clip, ecc_mode="loop")
+        if sd_ecc is None:
+            torch.manual_seed(1)
+            model = create_model(self.margs)
+            sd_ecc, sd_ptn = model.ecc.state_dict(), model.ptn.state_dict()
+        self.pcfg, self.mcfg = workloads.oracle_cfg(self.margs)
+        self.impl = nets_ref.RefTrainer(sd_ptn, sd_ecc, self.pcfg, self.mcfg, lr=self.margs.lr,
+                                        grad_clip=self.margs.grad_clip, ecc_mode="loop")
 
     def step(self, batch):
         """-> (loss | None, logits)"""
         if self.w["train"]:
-            if self.kind == "reference":
-                try:
-                    return self.impl.train_step(batch)
-                except RuntimeError as ex:
-                    # the reference's matrix-filter backward does not run on torch >= 2 (index_add_ shape
-                    # check at learning/ecc/GraphConvModule.py:146, SURVEY.md 8(c)): time the oracle port
-                    if "source tensor shape must match" not in str(ex):
-                        raise
-                    self.kind, self.note = "port", ("the reference's matrix-filter backward fails on torch>=2 "
-                                                    "(ecc/GraphConvModule.py:146): oracle port timed instead")
-                    self._make()
             return self.impl.step(batch)
-        if self.kind == "reference":
-            return None, self.impl.eval_step(batch)
         from oracle import nets_ref
         with torch.no_grad():
             return None, nets_ref.spg_forward(batch, self.impl.sd_ptn, self.impl.sd_ecc, self.pcfg, self.mcfg,
                                               False, ecc_mode="loop")
 
     def describe(self):
-        if getattr(self, "note", None):
-            return "oracle port of the reference CPU path (oracle/nets_ref, ecc_mode=loop); " + self.note
-        if self.kind == "reference":
-            return ("the reference's own modules (baseline/_ref: learning/pointnet.py, graphnet.py, modules.py, "
-                    "ecc/*; use_pyg=0, cuda=False) through CloudEmbedder.run / GraphNetwork / cross_entropy / "
-                    "clamp / Adam")
         return "oracle port of the reference CPU path (oracle/nets_ref, ecc_mode=loop)"
 
     def pick_threads(self, batch, budget_s=20.0):
@@ -374,7 +353,7 @@ def parity_check(w, batch, sd_ecc, sd_ptn, loss, logits):
 
 def ncu_traffic():
     """Per-launch DRAM traffic of the dominant kernels from the committed ncu captures
-    (profiles/ncu_traffic.json); {} if the file is missing."""
+    (profiles/ncu_traffic.json); {} if the file is missing (no capture is stored for the H100)."""
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")
     try:
         with open(path) as f:
@@ -503,6 +482,32 @@ def loader_roofline(dev, pk, with_cpu):
     return out
 
 
+def host_outputs(out):
+    """(loss | None, logits) of one step -> {name: float32 host array}; None when no step ran."""
+    if out is None:
+        return None
+    loss, logits = out
+    d = {"logits": logits.detach().float().cpu().numpy()}
+    if loss is not None:
+        d["loss"] = loss.detach().float().cpu().numpy().reshape(-1)[:1]
+    return d
+
+
+def dump_outputs(path, arrays, limit_bytes=64 << 20):
+    """DIR/<name>.npy for every output; a larger-than-limit array is replaced by a fixed, seeded row sample."""
+    if arrays is None:
+        raise RuntimeError("--dump-outputs needs at least one timed step (--steps >= 1)")
+    os.makedirs(path, exist_ok=True)
+    budget = limit_bytes // max(1, len(arrays))
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        if a.nbytes > budget:
+            rows = np.sort(np.random.RandomState(0).choice(a.shape[0], budget // (a.nbytes // a.shape[0]),
+                                                           replace=False))
+            a = a[rows]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def run_b200(args):
     import torch.distributed as dist
 
@@ -574,15 +579,17 @@ def run_b200(args):
     evs = []
     done_units = 0
     t_wall = time.perf_counter()
+    last = None
     for i in range(args.steps):
         flush.zero_()  # L2 flush, outside the event bracket
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
-        step(dbs[i % nb])
+        last = step(dbs[i % nb])
         e.record()
         evs.append((s, e))
         done_units += units[i % nb]
     barrier()
+    dumped = host_outputs(last)
     wall = time.perf_counter() - t_wall
     clocks = sampler.stop()
     launches = ops.total_launches() - launches0
@@ -615,11 +622,12 @@ def run_b200(args):
                 flush.zero_()
                 s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 s.record()
-                trainer.replay(graph_keys[i % nb])
+                last = trainer.replay(graph_keys[i % nb])
                 e.record()
                 evs.append((s, e))
                 done_units += units[i % nb]
             barrier()
+            dumped = host_outputs(last)  # (graph outputs are static buffers: copied before the next replay)
             wall = time.perf_counter() - t_wall
             clocks = sampler.stop()
             launches = launches_per_step * args.steps
@@ -652,11 +660,12 @@ def run_b200(args):
                 flush.zero_()
                 s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 s.record()
-                trainer.replay_eval(eval_keys[i % nb])
+                last = None, trainer.replay_eval(eval_keys[i % nb])
                 e.record()
                 evs.append((s, e))
                 done_units += units[i % nb]
             barrier()
+            dumped = host_outputs(last)
             wall = time.perf_counter() - t_wall
             clocks = sampler.stop()
             launches = launches_per_step * args.steps
@@ -670,6 +679,9 @@ def run_b200(args):
             value = all_units / (total_ms * 1e-3)
         except Exception as ex:  # keep the eager numbers
             eval_keys, graph_err = None, repr(ex)
+
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dumped)
 
     # ---- end-to-end through the public API with host buffers (H2D + step + D2H of loss/logits)
     h2d = hbs[0].h2d_bytes()
@@ -755,12 +767,13 @@ def run_b200(args):
                       "tc_gemm_3xtf32": ops.TC_FLOPS[0], "tc_dw_3xtf32": ops.DW_FLOPS[0],
                       "pointnet_fused_eval": ops.FUSED_FLOPS[0]}
             notes = {"gemm_f32": "exact-fp32 FMA GEMM (small/odd shapes), measured against the bf16 tensor peak",
-                     "tc_gemm_3xtf32": "tcgen05 kind::tf32, 3 MMAs per product (error-compensated split, fp32-"
+                     "tc_gemm_3xtf32": "wgmma tf32, 3 MMAs per product (error-compensated split, fp32-"
                                        "equivalent): algorithmic FLOPs counted once; ceiling = bf16 peak / 6",
-                     "tc_dw_3xtf32": "tcgen05 kind::tf32 MN-major operands, 3 MMAs per product; ceiling = bf16 peak / 6",
-                     "pointnet_fused_eval": ("fused eval trunk, tcgen05 kind::f16 on bf16 operands: ceiling = bf16 peak"
+                     "tc_dw_3xtf32": "wgmma tf32, operands transposed to K-major while staged, 3 MMAs per product; "
+                                     "ceiling = bf16 peak / 6",
+                     "pointnet_fused_eval": ("fused eval trunk, wgmma on bf16 operands: ceiling = bf16 peak"
                                              if w["dtype"] == "bf16" else
-                                             "fused eval trunk, tcgen05 kind::tf32, 3 MMAs per product (fp32-equivalent): "
+                                             "fused eval trunk, wgmma tf32, 3 MMAs per product (fp32-equivalent): "
                                              "algorithmic FLOPs counted once; ceiling = bf16 peak / 6")}
             dense = {}
             for name in ("tc_gemm_3xtf32", "tc_dw_3xtf32", "gemm_f32", "pointnet_fused_eval"):

@@ -2,12 +2,12 @@
 
     python compat/run_main.py [--reference-root DIR] -- <arguments of learning/main.py>
 
-* `superpoint_graph_b200.dropin.install()` registers the sm_100a mirrors under the reference's module
+* `superpoint_graph_b200.dropin.install()` registers the sm_90a mirrors under the reference's module
   names (learning.pointnet / graphnet / modules / ecc) before main.py's imports run;
 * packages the image lacks (igraph, h5py, torchnet, transforms3d) resolve to the stand-ins in this
   directory — only if the real ones cannot be imported;
-* main.py itself is executed with runpy from the reference checkout (default: /root/reference, else the
-  verbatim copy under baseline/_ref), byte for byte as it lies there.
+* main.py itself is executed with runpy from the reference checkout (--reference-root, else the
+  SPG_REFERENCE environment variable), byte for byte as it lies there.
 """
 import importlib
 import os
@@ -34,10 +34,10 @@ def _use_standins():
 
 
 def reference_root(explicit=None):
-    for cand in (explicit, os.environ.get("SPG_REFERENCE"), "/root/reference", os.path.join(ROOT, "baseline", "_ref")):
+    for cand in (explicit, os.environ.get("SPG_REFERENCE")):
         if cand and os.path.exists(os.path.join(cand, "learning", "main.py")):
             return cand
-    raise RuntimeError("no reference checkout with learning/main.py found (run baseline/install_ref.py)")
+    raise RuntimeError("no reference checkout with learning/main.py found (pass its path or set SPG_REFERENCE)")
 
 
 def run(main_args, ref_root=None):

@@ -1,5 +1,5 @@
 /*
- * spg_b200.h — C-ABI of libspg_b200.so, the sm_100a implementation of the
+ * spg_b200.h — C-ABI of libspg_b200.so, the sm_90a (H100) implementation of the
  * superpoint-graph learning hot path of loicland/superpoint_graph.
  *
  * Every entry point is `extern "C"`, takes plain device pointers, sizes and the
@@ -185,8 +185,8 @@ int spg_colstats_merge_fold(float* partials, int64_t n_partials, int C, float* m
 /* (the merge is two-level: `partials` needs room for ceil(n_partials/256) extra triples per column
  *  after the n_partials*C*3 floats; the same holds for the workspaces of spg_colstats / stats_ws) */
 
-/* tcgen05 tensor-core path of the same product for the large point-wise layers:
- *   C[M,N] = f(A)[M,K] * B[N,K]^T + bias in fp32-equivalent precision (3xTF32 split, fp32 TMEM
+/* wgmma tensor-core path of the same product for the large point-wise layers:
+ *   C[M,N] = f(A)[M,K] * B[N,K]^T + bias in fp32-equivalent precision (3xTF32 split, fp32 register
  *   accumulation), lda/ldc % 4 == 0, 16-byte aligned pointers.
  * B is given as a pre-split, pre-swizzled image built by spg_tc_pack_weights from W (ld = ldw):
  *   transpose=0: B[n][k] = W[n][k] (forward, W = [N,K]); transpose=1: B[n][k] = W[k][n]
@@ -243,7 +243,7 @@ int spg_tc_gemm_ex(const float* A, int64_t lda, const float* weight_image, const
 /* Weight gradient of a point-wise layer on the tensor cores (3xTF32, fp32-equivalent):
  *   dW[co,ci] = sum_m dY[m,co] * f(P)[m,ci],  f = affine(p_scale,p_shift)+ReLU of P's producer.
  * co in {64,128,256}, ci in {32,64,128}; every CTA reduces a slab of points into a partial held in
- * TMEM, workspace >= spg_tc_dw_ctas(M)*co*ci floats, partials are summed in a fixed order.
+ * registers, workspace >= spg_tc_dw_ctas(M)*co*ci floats, partials are summed in a fixed order.
  * C[M,N] = sum_z partials[z,M,N] (+ bias) is also exported on its own (spg_splitk_reduce).       */
 int spg_tc_dw_supported(int64_t M, int co, int ci);
 int spg_tc_dw_ctas(int64_t M);
@@ -409,8 +409,8 @@ int spg_allreduce_clamp_adam(const float* grad, float* const* peer_stage, uint32
  *   if T: (x0, x1) <- (x0, x1) (T[b] (+ I))                                   (pointnet.py:123)
  *   for l < n_layers: x <- relu(W_l x + b_l)     W_l [widths[l], K_l], BatchNorm already folded in
  *   pooled[b, :widths[n_layers-1]] = max over the 128 points
- * Activations stay in shared memory / TMEM; the input tile and the weight stream arrive by TMA;
- * products are 3xTF32 on tcgen05 (fp32-equivalent).  weight_image = for each layer the
+ * Activations stay in shared memory; the input tile and the weight stream arrive by TMA;
+ * products are 3xTF32 on wgmma (fp32-equivalent).  weight_image = for each layer the
  * spg_tc_pack_weights_scaled image ([K_l/32][hi|lo][N_l][32 floats]; K_0 = 32, k_valid = F) back to
  * back (spg_pointnet_fused_image_rows(...) * 32 floats); bias = the folded biases back to back;
  * widths: HOST int32 array, every width in {32,64,128,256}, inner widths <= 128, at most 6 layers.   */
@@ -419,8 +419,8 @@ int64_t spg_pointnet_fused_image_rows(int n_features, int n_layers, const int32_
 int spg_pointnet_fused_eval(const float* clouds, int64_t n_clouds, int n_features, int n_points, const float* T,
                             int add_eye, const float* weight_image, const float* bias, int n_layers,
                             const int32_t* widths, float* pooled, int64_t ldp, spg_stream_t stream);
-/* bf16 arithmetic for the same trunk (BASELINE configs[3]): bf16 operands, fp32 accumulation in TMEM
- * (tcgen05.mma kind::f16, one MMA per product), activations between layers as bf16 on chip; inputs
+/* bf16 arithmetic for the same trunk (BASELINE configs[3]): bf16 operands, fp32 accumulation in registers
+ * (wgmma bf16, one MMA per product), activations between layers as bf16 on chip; inputs
  * fp32 [B,F,128], pooled output fp32.  weight_image: per layer [K_l/64][N_l][64] bf16 from
  * spg_tc_pack_weights_bf16 (K_0 = 64 with k_valid = F; a layer that follows a 32-wide one has K = 64 with
  * k_valid = 32).  Agreement with the fp32 path is bounded by bf16 rounding (~1e-2), not 1e-4.          */

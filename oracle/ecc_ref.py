@@ -2,7 +2,7 @@
 
 CPU restatement of the reference's edge-conditioned convolution and its host-side graph
 bookkeeping.  Pinned against the reference itself: tests/golden/make_golden.py imports
-/root/reference in the build container and stores its outputs, tests/test_oracle_golden.py checks
+the reference checkout (SPG_REFERENCE) and stores its outputs, tests/test_oracle_golden.py checks
 this file against them.
 
 Each function cites the reference lines it restates (paths relative to the reference root).

@@ -1,4 +1,4 @@
-"""superpoint_graph_b200 — sm_100a implementation of the superpoint-graph learning hot path
+"""superpoint_graph_b200 — sm_90a (H100) implementation of the superpoint-graph learning hot path
 (PointNet embedding + edge-conditioned convolution + GRU cell) behind the reference's own
 `learning/pointnet`, `learning/ecc`, `learning/modules`, `learning/graphnet` operator API.
 

@@ -1,4 +1,4 @@
-"""In-tree build of libspg_b200.so (sm_100a only, nvcc cross-compiles without a GPU).
+"""In-tree build of libspg_b200.so (sm_90a only, nvcc cross-compiles without a GPU).
 
     python -m superpoint_graph_b200.build [--force]
 
@@ -17,7 +17,7 @@ OBJ_DIR = os.path.join(ROOT, "build", "obj")
 LIB_PATH = os.path.join(HERE, "libspg_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",

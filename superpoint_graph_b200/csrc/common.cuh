@@ -1,4 +1,4 @@
-// Shared helpers for libspg_b200 (sm_100a only).
+// Shared helpers for libspg_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -65,7 +65,7 @@ struct LaunchScope {
 // cudaGetLastError() -> return code of the C-ABI call.
 inline int launch_status() { return (int)cudaGetLastError(); }
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;  // H100 SXM
 
 __host__ __device__ inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
@@ -100,7 +100,7 @@ bool vec_affine_act(const float* Y, int64_t ldy, const float* scale, const float
 // Programmatic dependent launch (sm_90+): every kernel of this library starts with pdl_entry() — wait until
 // the kernels it depends on have completed and flushed, then allow the NEXT kernel of the stream to be
 // scheduled — and is launched with programmaticStreamSerialization, so that the launch latency, block
-// scheduling and pre-wait set-up (barrier init, tensor-memory allocation) of kernel n+1 overlap kernel n.
+// scheduling and pre-wait set-up (barrier init, descriptor prefetch) of kernel n+1 overlap kernel n.
 // The trigger comes AFTER the wait on purpose: at most one dependent grid is resident and waiting.
 // spg_set_pdl(0) switches the attribute off (plain stream order; the device instructions are then no-ops).
 #define SPG_PDL_ENTRY()                                          \

@@ -9,7 +9,7 @@
 // stored and the normalisation + activation happen while the next GEMM loads it.
 //
 // This file is the exact-fp32 engine (parity reference on device and the path for
-// small / odd shapes).  The large point-wise layers are served by the tcgen05
+// small / odd shapes).  The large point-wise layers are served by the wgmma
 // 3xTF32 kernel in tc_gemm.cu when it applies.
 #include "common.cuh"
 

@@ -1,7 +1,7 @@
 // Eval-mode PointNet trunk as ONE kernel per chain: cloud tile -> (xy transform) -> up to six point-wise
 // layers (Conv1d k=1 with BatchNorm folded into weights and bias, ReLU) -> max over the cloud's points.
-// No [rows, C] activation ever reaches HBM: a CTA keeps one superpoint (128 points = one UMMA M tile) on
-// chip from the input tile to the pooled row.
+// No [rows, C] activation ever reaches HBM: a CTA keeps one superpoint (128 points) on chip from the input
+// tile to the pooled row.
 //
 //   reference: learning/pointnet.py:120-133 (PointNet.forward) and :55-61 (STNkD.forward) under
 //   model.eval() (learning/main.py:229-311): conv -> BatchNorm1d(running statistics) -> ReLU chains, then
@@ -9,18 +9,20 @@
 //
 // Per CTA (persistent over superpoints b = blockIdx.x, blockIdx.x + gridDim.x, ...):
 //   warp 8 (one thread)  TMA producer: the superpoint's [F, 128] input tile (cp.async.bulk.tensor over the
-//                        NCL clouds tensor) and the weight stream — for every layer, N-tile and 32-float
-//                        K-chunk one [N_tile x 128 B] hi block and one lo block of the pre-split,
-//                        pre-swizzled weight image (the weights live in L2; 2-stage ring of 32 KB)
-//   warp 9 (one thread)  MMA issuer: tcgen05.mma kind::tf32, 3 MMAs per product (3xTF32: fp32-equivalent),
-//                        A = the layer's input activations in shared memory (K-major SWIZZLE_128B hi/lo),
-//                        B = the weight stage, D = TMEM accumulator (one 128-column tile per N-tile)
-//   warps 0-7            one thread per (point, half of the channel blocks): input tile -> transform -> tf32 split -> A; after every
-//                        layer tcgen05.ld of the accumulator row, + folded bias, ReLU, tf32 split, written
-//                        IN PLACE as the next layer's A operand; after the last layer the max over the 128
-//                        points (redux.sync on the non-negative float bits) -> pooled[b, :]
-// mbarriers: w_full/w_empty (weight ring), x_full/x_empty (input double buffer), a_ready (A operand of the
-// next layer is in shared memory), acc_full[t] (all MMAs of N-tile t have completed).
+//                        NCL clouds tensor) and the weight stream — for every layer, N-tile and K-chunk one
+//                        [N_tile x 128 B] block (fp32 path: a hi and a lo block) of the pre-split,
+//                        pre-swizzled weight image (the weights live in L2)
+//   warps 0-7            two consumer warpgroups, one per 64 points: input tile -> transform -> A chunk 0;
+//                        per layer wgmma.mma_async with A = the layer's input activations in shared memory
+//                        (K-major SWIZZLE_128B, the warpgroup's own 64 rows) and B = the weight stage, fp32
+//                        accumulator in registers; then + folded bias, ReLU, written IN PLACE as the next
+//                        layer's A (every MMA of the layer has completed first: a non-last layer is one
+//                        N-tile); after the last layer the max over the points -> pooled[b, :]
+// fp32 path: 3xTF32 (hi/lo split of both operands, three MMAs per product: fp32-equivalent).
+// bf16 path (configs[3] arithmetic): bf16 operands, fp32 accumulation, ONE MMA per product; inputs and every
+// layer output are rounded to bf16 (8-bit mantissa): results agree with the fp32 path to ~1e-2 (tests state
+// the bound), not to 1e-4.
+// mbarriers: w_full/w_empty (weight ring), x_full/x_empty (input double buffer).
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -31,32 +33,37 @@
 
 namespace spg {
 
-constexpr int PF_ROWS = 128;          // points per superpoint = UMMA M
+constexpr int PF_ROWS = 128;          // points per superpoint
 constexpr int PF_KC = 32;             // floats per K chunk (one 128-byte swizzle row)
 constexpr int PF_MAXK = 128;          // widest layer input kept in shared memory
-constexpr int PF_NT = 128;            // accumulator tile width (TMEM columns per N-tile).  (64-column tiles would let
-                                      // the activation warps drain tile t under the MMAs of tile t+1, but the next A
-                                      // operand is written IN PLACE: every MMA of the layer must have finished first)
-constexpr int PF_MAX_TILES = 2;
-constexpr int PF_STAGES_TMEM_A = 6;   // weight ring depth (32 KB stages); the A operand lives in tensor memory
+constexpr int PF_NT = 128;            // accumulator tile width
 constexpr int PF_STAGE_BYTES = 2 * PF_NT * PF_KC * 4;        // hi + lo of one (N-tile, K-chunk) = 32 KB
+constexpr int PF_STAGES = 2;          // fp32 weight ring depth (the 128 KB hi|lo A operand takes the rest)
+constexpr int PF_A_CHUNK_BYTES = PF_ROWS * 128;              // one 128-byte-row K chunk of A: 16 KB
+constexpr int PF_A_BYTES = (PF_MAXK / PF_KC) * PF_A_CHUNK_BYTES;  // 64 KB (hi or lo)
 constexpr int PF_MAXF = 16;            // input features (S3DIS 14, Semantic3D 11, vKITTI 9)
 constexpr int PF_X_BYTES = PF_MAXF * PF_ROWS * 4;            // one input tile buffer (8 KB)
 constexpr int PF_MAX_LAYERS = 6;
-constexpr int PF_ACT_WARPS = 8;        // activation warps: two per TMEM lane quarter (alternate 32-column blocks)
-constexpr int PF_THREADS = (PF_ACT_WARPS + 2) * 32;
+constexpr int PF_ACT_WARPS = 8;        // consumer warps: two warpgroups
+constexpr int PF_THREADS = (PF_ACT_WARPS + 1) * 32;
 constexpr int PF_MAX_BIAS = 1024;
+constexpr int PF_POOL_FLOATS = PF_ACT_WARPS * 256;
+
+constexpr int PB_KC = 64;                                   // bf16 elements per K chunk (128-byte row)
+constexpr int PB_STAGES = 8;
+constexpr int PB_STAGE_BYTES = PF_NT * 128;                 // one (N-tile, K-chunk) weight block = 16 KB
+constexpr int PB_A_BYTES = (PF_MAXK / PB_KC) * PF_A_CHUNK_BYTES;  // 32 KB
 
 struct PfLayer {
-    int K, N;      // K padded to a multiple of 32, N in {64, 128, 256}
-    int w_row;     // first row of this layer's blocks in the weight image ([rows][32 floats])
+    int K, N;      // K padded to a multiple of the chunk, N in {32, 64, 128, 256}
+    int w_row;     // first row of this layer's blocks in the weight image ([rows][128 B])
     int b_off;     // offset of the folded bias in the bias vector
 };
 
 struct PfArgs {
     int n_layers;
     PfLayer L[PF_MAX_LAYERS];
-    int F;                 // input features (<= 32)
+    int F;                 // input features (<= 16)
     int64_t B;             // superpoints
     const float* T;        // [B, 4] spatial transformer output (xy' = xy (T + I)), or null
     int add_eye;
@@ -66,12 +73,6 @@ struct PfArgs {
     int64_t ldp;
 };
 
-__device__ __forceinline__ void pf_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void pf_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void pf_tma_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
@@ -79,74 +80,159 @@ __device__ __forceinline__ void pf_tma_2d(uint32_t dst, const CUtensorMap* map, 
         : "memory");
 }
 
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
+__device__ __forceinline__ uint32_t pack_bf16x2(float e0, float e1) {  // e0 -> low half (lower address)
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(e1), "f"(e0));
+    return r;
 }
 
-// The A operand (the layer's input activations, tf32 hi | lo) lives in TENSOR MEMORY: the activation warps
-// write the row they own with tcgen05.st (TMEM lane = point, column = channel — the layout the accumulator
-// row already has, no shared-memory transposition), the MMA reads it directly, and all of shared memory goes
-// to a 6-stage weight ring.  TMEM columns: [0,256) accumulators, [256,384) A hi, [384,512) A lo.
-// (A shared-memory A operand — K-major SWIZZLE_128B, 128 KB, 2-stage ring — was measured 7 % slower.)
+__device__ __forceinline__ void bar_named(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+template <bool BF16>
+struct PfCfg {
+    static constexpr int KC = BF16 ? PB_KC : PF_KC;
+    static constexpr int STAGES = BF16 ? PB_STAGES : PF_STAGES;
+    static constexpr int STAGE_BYTES = BF16 ? PB_STAGE_BYTES : PF_STAGE_BYTES;
+    static constexpr int A_BYTES = BF16 ? PB_A_BYTES : 2 * PF_A_BYTES;  // fp32: [hi][lo]
+    static constexpr int SMEM = A_BYTES + STAGES * STAGE_BYTES + 2 * PF_X_BYTES + (PF_MAX_BIAS + PF_POOL_FLOATS) * 4;
+};
+
+// Shared-memory state one consumer warpgroup works with.
+struct PfCtx {
+    uint32_t a_u, w_u, bars_u;
+    float* bias_s;
+    float* pool_s;
+    int g, warp, lane;
+};
+
+// One N-tile of one layer for the calling warpgroup: MMAs over the weight stream, then the epilogue.
+template <bool BF16, int NT>
+__device__ __forceinline__ void pf_tile(const PfCtx& c, const PfLayer& Ly, int nt, bool last, uint32_t& it) {
+    using C = PfCfg<BF16>;
+    float acc[NT / 2];
+    const uint32_t a_rows = c.a_u + (uint32_t)c.g * (64 * 128);  // this warpgroup's 64 rows of every A chunk
+    for (int kc = 0; kc < Ly.K / C::KC; ++kc, ++it) {
+        const int s = it % C::STAGES;
+        mbar_wait(c.bars_u + 8u * (uint32_t)s, (it / C::STAGES) & 1);  // w_full(s)
+        const uint32_t a0 = a_rows + (uint32_t)kc * PF_A_CHUNK_BYTES;
+        const uint32_t b0 = c.w_u + (uint32_t)s * C::STAGE_BYTES;
+        wg_reg_fence(acc);
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {  // 32 bytes of the 128-byte row per instruction
+            const uint32_t ko = ks * 32;
+            if constexpr (BF16) {
+                wgmma_bf16<NT>(acc, wg_desc_k_sw128(a0 + ko), wg_desc_k_sw128(b0 + ko), (kc | ks) ? 1u : 0u);
+            } else {
+                const uint64_t dah = wg_desc_k_sw128(a0 + ko), dal = wg_desc_k_sw128(a0 + PF_A_BYTES + ko);
+                const uint64_t dbh = wg_desc_k_sw128(b0 + ko), dbl = wg_desc_k_sw128(b0 + NT * 128 + ko);
+                wgmma_tf32<NT>(acc, dah, dbh, (kc | ks) ? 1u : 0u);
+                wgmma_tf32<NT>(acc, dal, dbh, 1u);
+                wgmma_tf32<NT>(acc, dah, dbl, 1u);
+            }
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_reg_fence(acc);
+        __syncwarp();
+        if (c.lane == 0) mbar_arrive(c.bars_u + 8u * (uint32_t)(C::STAGES + s));  // w_empty(s)
+    }
+    // this thread holds points prow and prow + 8, columns 8j + cq, 8j + cq + 1 of the tile
+    const int r = c.lane >> 2, cq = 2 * (c.lane & 3);
+    const int prow = c.g * 64 + (c.warp & 3) * 16 + r;
+    const float* bs = c.bias_s + Ly.b_off + nt * NT;
+    if (!last) {
+        // in place: every warp of the warpgroup has finished reading this layer's A
+        bar_named(1 + c.g, 128);
+#pragma unroll
+        for (int j = 0; j < NT / 8; ++j) {
+            const int col = 8 * j + cq;  // a non-last layer is a single N-tile: col is the channel
+            const float o0 = fmaxf(acc[4 * j] + bs[col], 0.f), o1 = fmaxf(acc[4 * j + 1] + bs[col + 1], 0.f);
+            const float o2 = fmaxf(acc[4 * j + 2] + bs[col], 0.f), o3 = fmaxf(acc[4 * j + 3] + bs[col + 1], 0.f);
+            if constexpr (BF16) {
+                const uint32_t base = c.a_u + (uint32_t)(col / PB_KC) * PF_A_CHUNK_BYTES + (uint32_t)(col & 7) * 2u;
+                const int c16 = (col % PB_KC) >> 3;
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(base + sw128_off(prow, c16)), "r"(pack_bf16x2(o0, o1)) : "memory");
+                asm volatile("st.shared.b32 [%0], %1;" ::"r"(base + sw128_off(prow + 8, c16)), "r"(pack_bf16x2(o2, o3)) : "memory");
+                if (NT == 32) {  // a 32-wide layer fills only half of the next 64-element K chunk: zero the rest
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(base + sw128_off(prow, c16 + 4)), "r"(0u) : "memory");
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(base + sw128_off(prow + 8, c16 + 4)), "r"(0u) : "memory");
+                }
+            } else {
+                const uint32_t base = c.a_u + (uint32_t)(col / PF_KC) * PF_A_CHUNK_BYTES + (uint32_t)(col & 3) * 4u;
+                const int c16 = (col % PF_KC) >> 2;
+                const float ov[4] = {o0, o1, o2, o3};
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const uint32_t addr = base + sw128_off(prow + 8 * h, c16);
+                    const uint32_t h0 = to_tf32(ov[2 * h]), h1 = to_tf32(ov[2 * h + 1]);
+                    const uint32_t l0 = to_tf32(ov[2 * h] - __uint_as_float(h0));
+                    const uint32_t l1 = to_tf32(ov[2 * h + 1] - __uint_as_float(h1));
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(h0), "r"(h1) : "memory");
+                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr + PF_A_BYTES), "r"(l0), "r"(l1) : "memory");
+                }
+            }
+        }
+    } else {
+        // max over the points: the thread's two rows, then the 8 row pairs of the warp (lanes with the same
+        // lane % 4 hold the same columns); the 8 warps are folded after the last N-tile
+#pragma unroll
+        for (int j = 0; j < NT / 8; ++j) {
+            const int col = 8 * j + cq;
+            float m0 = fmaxf(fmaxf(acc[4 * j] + bs[col], 0.f), fmaxf(acc[4 * j + 2] + bs[col], 0.f));
+            float m1 = fmaxf(fmaxf(acc[4 * j + 1] + bs[col + 1], 0.f), fmaxf(acc[4 * j + 3] + bs[col + 1], 0.f));
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+                m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+                m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+            }
+            if (r == 0) {
+                c.pool_s[c.warp * 256 + nt * NT + col] = m0;
+                c.pool_s[c.warp * 256 + nt * NT + col + 1] = m1;
+            }
+        }
+    }
+}
+
+template <bool BF16>
 __global__ void __launch_bounds__(PF_THREADS, 1)
 pointnet_fused_kernel(const PfArgs p, const __grid_constant__ CUtensorMap wmap,
                       const __grid_constant__ CUtensorMap xmap) {
-    constexpr int PF_STAGES = PF_STAGES_TMEM_A;
-    constexpr uint32_t TM_COLS = 512u;
-    constexpr uint32_t TM_AHI = 256u, TM_ALO = 384u;
+    using C = PfCfg<BF16>;
     extern __shared__ __align__(1024) uint8_t smem[];
     if ((smem_u32(smem) & 1023u) != 0u) __trap();
-    // [weight ring 6 x 32 KB][input tiles 2 x 8 KB][bias][pool scratch]
-    uint8_t* w_s = smem;
-    uint8_t* x_s = w_s + PF_STAGES * PF_STAGE_BYTES;
+    // [A operand][weight ring][input tiles 2 x 8 KB][bias][pool scratch]
+    uint8_t* a_s = smem;
+    uint8_t* w_s = a_s + C::A_BYTES;
+    uint8_t* x_s = w_s + C::STAGES * C::STAGE_BYTES;
     float* bias_s = reinterpret_cast<float*>(x_s + 2 * PF_X_BYTES);
-    float* pool_s = bias_s + PF_MAX_BIAS;  // [4 warps][256]
-    __shared__ __align__(8) uint64_t bars[2 * PF_STAGES_TMEM_A + 4 + 1 + PF_MAX_TILES];
-    __shared__ uint32_t tmem_base_s;
+    float* pool_s = bias_s + PF_MAX_BIAS;  // [8 warps][256]
+    __shared__ __align__(8) uint64_t bars[2 * PB_STAGES + 4];
 
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
     const uint32_t bars_u = smem_u32(&bars[0]);
     auto w_full = [&](int s) { return bars_u + 8u * (uint32_t)s; };
-    auto w_empty = [&](int s) { return bars_u + 8u * (uint32_t)(PF_STAGES + s); };
-    auto x_full = [&](int s) { return bars_u + 8u * (uint32_t)(2 * PF_STAGES + s); };
-    auto x_empty = [&](int s) { return bars_u + 8u * (uint32_t)(2 * PF_STAGES + 2 + s); };
-    const uint32_t a_ready = bars_u + 8u * (2 * PF_STAGES + 4);
-    auto acc_full = [&](int nt) { return bars_u + 8u * (uint32_t)(2 * PF_STAGES + 5 + nt); };
+    auto w_empty = [&](int s) { return bars_u + 8u * (uint32_t)(C::STAGES + s); };
+    auto x_full = [&](int s) { return bars_u + 8u * (uint32_t)(2 * C::STAGES + s); };
+    auto x_empty = [&](int s) { return bars_u + 8u * (uint32_t)(2 * C::STAGES + 2 + s); };
 
     if (t == 0) {
-        for (int s = 0; s < PF_STAGES; ++s) {
+        for (int s = 0; s < C::STAGES; ++s) {
             mbar_init(w_full(s), 1);
-            mbar_init(w_empty(s), 1);
+            mbar_init(w_empty(s), PF_ACT_WARPS);
         }
         for (int s = 0; s < 2; ++s) {
             mbar_init(x_full(s), 1);
             mbar_init(x_empty(s), PF_ACT_WARPS);
         }
-        for (int s = 0; s < PF_MAX_TILES; ++s) mbar_init(acc_full(s), 1);
-        mbar_init(a_ready, PF_ACT_WARPS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                         smem_u32(&tmem_base_s)), "r"(TM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     SPG_PDL_ENTRY();  // set-up above overlaps the previous kernel of the stream; global memory only below
     for (int i = t; i < p.n_bias; i += PF_THREADS) bias_s[i] = p.bias[i];
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
-    const uint32_t w_u = smem_u32(w_s), x_u = smem_u32(x_s);
+    const uint32_t a_u = smem_u32(a_s), w_u = smem_u32(w_s), x_u = smem_u32(x_s);
 
     if (warp == PF_ACT_WARPS) {
         // ================================ TMA producer ================================
@@ -157,78 +243,53 @@ pointnet_fused_kernel(const PfArgs p, const __grid_constant__ CUtensorMap wmap,
             for (int64_t b = blockIdx.x; b < p.B; b += gridDim.x, ++ci) {
                 const int xb = ci & 1;
                 mbar_wait(x_empty(xb), ((ci >> 1) & 1) ^ 1);
-                pf_expect_tx(x_full(xb), (uint32_t)(p.F * PF_ROWS * 4));
+                mbar_expect_tx(x_full(xb), (uint32_t)(p.F * PF_ROWS * 4));
                 pf_tma_2d(x_u + xb * PF_X_BYTES, &xmap, 0, (int)(b * p.F), x_full(xb));
                 for (int l = 0; l < p.n_layers; ++l) {
                     const PfLayer& Ly = p.L[l];
                     const int ntile = Ly.N < PF_NT ? Ly.N : PF_NT;
                     for (int nt = 0; nt < Ly.N / ntile; ++nt)
-                        for (int kc = 0; kc < Ly.K / PF_KC; ++kc, ++it) {
-                            const int s = it % PF_STAGES;
-                            mbar_wait(w_empty(s), ((it / PF_STAGES) & 1) ^ 1);
-                            pf_expect_tx(w_full(s), (uint32_t)(2 * ntile * PF_KC * 4));
-                            const uint32_t dst = w_u + s * PF_STAGE_BYTES;
-                            // image rows of this layer: [(kc*2 + half)*N + n]
-                            for (int half = 0; half < 2; ++half)
-                                for (int sub = 0; sub < ntile / 32; ++sub)  // TMA boxes of 32 rows
-                                    pf_tma_2d(dst + (uint32_t)(half * ntile + sub * 32) * (PF_KC * 4), &wmap, 0,
-                                              Ly.w_row + (kc * 2 + half) * Ly.N + nt * ntile + sub * 32, w_full(s));
-                        }
-                }
-            }
-        }
-    } else if (warp == PF_ACT_WARPS + 1) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            uint32_t it = 0, q = 0;
-            for (int64_t b = blockIdx.x; b < p.B; b += gridDim.x) {
-                for (int l = 0; l < p.n_layers; ++l, ++q) {
-                    const PfLayer& Ly = p.L[l];
-                    const int ntile = Ly.N < PF_NT ? Ly.N : PF_NT;
-                    const uint32_t idesc = umma_idesc_tf32(PF_ROWS, ntile);
-                    mbar_wait(a_ready, q & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    for (int nt = 0; nt < Ly.N / ntile; ++nt) {
-                        const uint32_t d = tmem_base + (uint32_t)(nt * PF_NT);
-                        for (int kc = 0; kc < Ly.K / PF_KC; ++kc, ++it) {
-                            const int s = it % PF_STAGES;
-                            mbar_wait(w_full(s), (it / PF_STAGES) & 1);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                            const uint32_t b_hi = w_u + (uint32_t)s * PF_STAGE_BYTES;
-                            const uint32_t b_lo = b_hi + (uint32_t)ntile * PF_KC * 4;
-#pragma unroll
-                            for (int ks = 0; ks < PF_KC / 8; ++ks) {
-                                const uint32_t ko = ks * 32;
-                                const uint64_t dbh = umma_desc_k_sw128(b_hi + ko), dbl = umma_desc_k_sw128(b_lo + ko);
-                                const uint32_t th = tmem_base + TM_AHI + (uint32_t)(kc * PF_KC + ks * 8);
-                                const uint32_t tl = tmem_base + TM_ALO + (uint32_t)(kc * PF_KC + ks * 8);
-                                umma_tf32_ts(d, th, dbh, idesc, (kc | ks) ? 1u : 0u);
-                                umma_tf32_ts(d, tl, dbh, idesc, 1u);
-                                umma_tf32_ts(d, th, dbl, idesc, 1u);
+                        for (int kc = 0; kc < Ly.K / C::KC; ++kc, ++it) {
+                            const int s = it % C::STAGES;
+                            mbar_wait(w_empty(s), ((it / C::STAGES) & 1) ^ 1);
+                            const uint32_t dst = w_u + s * C::STAGE_BYTES;
+                            if constexpr (BF16) {
+                                mbar_expect_tx(w_full(s), (uint32_t)(ntile * 128));
+                                // image rows of this layer: [kc*N + n], 128 bytes each; boxes of 32 rows
+                                for (int sub = 0; sub < ntile / 32; ++sub)
+                                    pf_tma_2d(dst + (uint32_t)(sub * 32 * 128), &wmap, 0,
+                                              Ly.w_row + kc * Ly.N + nt * ntile + sub * 32, w_full(s));
+                            } else {
+                                mbar_expect_tx(w_full(s), (uint32_t)(2 * ntile * 128));
+                                // image rows of this layer: [(kc*2 + half)*N + n]
+                                for (int half = 0; half < 2; ++half)
+                                    for (int sub = 0; sub < ntile / 32; ++sub)
+                                        pf_tma_2d(dst + (uint32_t)(half * ntile + sub * 32) * 128u, &wmap, 0,
+                                                  Ly.w_row + (kc * 2 + half) * Ly.N + nt * ntile + sub * 32, w_full(s));
                             }
-                            umma_commit(w_empty(s));
                         }
-                        umma_commit(acc_full(nt));
-                    }
                 }
             }
         }
-    } else {
-        // ======================= activation warps: one thread per point =======================
-        const int quarter = warp & 3, half = warp >> 2;  // TMEM lane quarter; which 32-column blocks
-        const int row = quarter * 32 + lane;             // 0..127 = TMEM lane = point of the superpoint
-        uint32_t ci = 0, acc_cnt[PF_MAX_TILES] = {0u, 0u};
+    } else if (warp < PF_ACT_WARPS) {
+        // ======================= consumer warpgroups: 64 points each =======================
+        PfCtx c;
+        c.a_u = a_u; c.w_u = w_u; c.bars_u = bars_u; c.bias_s = bias_s; c.pool_s = pool_s;
+        c.g = warp >> 2; c.warp = warp; c.lane = lane;
+        const int tw = t & 127;
+        const int row = c.g * 64 + (tw & 63), fh = tw >> 6;  // input point; features 16*fh .. 16*fh+15
+        uint32_t it = 0, ci = 0;
         for (int64_t b = blockIdx.x; b < p.B; b += gridDim.x, ++ci) {
-            // ---- input tile -> (xy transform) -> A chunk 0
+            // ---- input tile -> (xy transform) -> A chunk 0 (features, zero-padded to the chunk)
             const int xb = ci & 1;
             mbar_wait(x_full(xb), (ci >> 1) & 1);
             const float* xin = reinterpret_cast<const float*>(x_s + xb * PF_X_BYTES);
-            float v[PF_KC];  // one K chunk: the features, zero-padded to 32
+            float v[16];
 #pragma unroll
-            for (int f = 0; f < PF_KC; ++f) v[f] = (f < PF_MAXF && f < p.F) ? xin[f * PF_ROWS + row] : 0.f;
+            for (int f = 0; f < 16; ++f) v[f] = (fh == 0 && f < p.F) ? xin[f * PF_ROWS + row] : 0.f;
             __syncwarp();
-            if (lane == 0) pf_arrive(x_empty(xb));
-            if (p.T && p.F >= 2) {
+            if (lane == 0) mbar_arrive(x_empty(xb));
+            if (fh == 0 && p.T && p.F >= 2) {
                 const float eye = p.add_eye ? 1.f : 0.f;
                 const float t00 = p.T[b * 4 + 0] + eye, t01 = p.T[b * 4 + 1], t10 = p.T[b * 4 + 2],
                             t11 = p.T[b * 4 + 3] + eye;
@@ -236,312 +297,65 @@ pointnet_fused_kernel(const PfArgs p, const __grid_constant__ CUtensorMap wmap,
                 v[0] = fmaf(x0, t00, x1 * t10);  // row vector times T (pointnet.py:123)
                 v[1] = fmaf(x0, t01, x1 * t11);
             }
-            const uint32_t lane_base = tmem_base + ((uint32_t)(quarter * 32) << 16);
-            auto store_chunk = [&](int kc, const float (&o)[32]) {
-                // 32 consecutive channels of this thread's row = K chunk kc of the next A operand
-                uint32_t hi[32], lo[32];
+            if constexpr (BF16) {
+                // 64-element chunk: fh 0 writes 16-byte chunks 0-1 (features), fh 1 chunks 2-7 (zeros)
+                if (fh == 0) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    hi[j] = to_tf32(o[j]);
-                    lo[j] = to_tf32(o[j] - __uint_as_float(hi[j]));
+                    for (int q = 0; q < 2; ++q)
+                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a_u + sw128_off(row, q)),
+                                     "r"(pack_bf16x2(v[8 * q], v[8 * q + 1])), "r"(pack_bf16x2(v[8 * q + 2], v[8 * q + 3])),
+                                     "r"(pack_bf16x2(v[8 * q + 4], v[8 * q + 5])), "r"(pack_bf16x2(v[8 * q + 6], v[8 * q + 7]))
+                                     : "memory");
+                } else {
+#pragma unroll
+                    for (int q = 2; q < 8; ++q)
+                        asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(a_u + sw128_off(row, q)), "r"(0u)
+                                     : "memory");
                 }
-                tmem_st32(lane_base + TM_AHI + (uint32_t)(kc * PF_KC), hi);
-                tmem_st32(lane_base + TM_ALO + (uint32_t)(kc * PF_KC), lo);
-            };
-            auto publish_a = [&]() {
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) pf_arrive(a_ready);
-            };
-            if (half == 0) store_chunk(0, v);
-            publish_a();
+            } else {
+                // 32-float chunk: fh writes 16-byte chunks 4*fh .. 4*fh+3, hi and lo
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    uint32_t hi[4], lo[4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        hi[e] = to_tf32(v[4 * q + e]);
+                        lo[e] = to_tf32(v[4 * q + e] - __uint_as_float(hi[e]));
+                    }
+                    const uint32_t addr = a_u + sw128_off(row, 4 * fh + q);
+                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(hi[0]), "r"(hi[1]),
+                                 "r"(hi[2]), "r"(hi[3]) : "memory");
+                    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr + PF_A_BYTES), "r"(lo[0]),
+                                 "r"(lo[1]), "r"(lo[2]), "r"(lo[3]) : "memory");
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            bar_named(1 + c.g, 128);
             // ---- layers
             for (int l = 0; l < p.n_layers; ++l) {
                 const PfLayer& Ly = p.L[l];
                 const int ntile = Ly.N < PF_NT ? Ly.N : PF_NT;
                 const bool last = l + 1 == p.n_layers;
                 for (int nt = 0; nt < Ly.N / ntile; ++nt) {
-                    mbar_wait(acc_full(nt), acc_cnt[nt] & 1);
-                    ++acc_cnt[nt];
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    for (int cb = half; cb < ntile / 32; cb += PF_ACT_WARPS / 4) {
-                        uint32_t r[32];
-                        tmem_ld32(lane_base + (uint32_t)(nt * PF_NT + cb * 32), r);
-                        const int col0 = nt * ntile + cb * 32;
-                        const float* bs = bias_s + Ly.b_off + col0;
-                        if (!last) {
-                            // next layer's A operand: these 32 columns are exactly K chunk col0/32
-                            float o[32];
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) o[j] = fmaxf(__uint_as_float(r[j]) + bs[j], 0.f);
-                            store_chunk(col0 / PF_KC, o);
-                        } else {
-                            // max over the 32 points of this warp: ReLU output is >= 0, so the float order
-                            // is the unsigned order of the bit patterns (one redux.sync per column)
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                const float o = fmaxf(__uint_as_float(r[j]) + bs[j], 0.f);
-                                const unsigned m = __reduce_max_sync(0xffffffffu, __float_as_uint(o));
-                                if (lane == j) pool_s[quarter * 256 + col0 + j] = __uint_as_float(m);
-                            }
-                        }
-                    }
+                    if (ntile == 128) pf_tile<BF16, 128>(c, Ly, nt, last, it);
+                    else if (ntile == 64) pf_tile<BF16, 64>(c, Ly, nt, last, it);
+                    else pf_tile<BF16, 32>(c, Ly, nt, last, it);
                 }
                 if (!last) {
-                    // (all MMAs that read the old A have completed: acc_full of every N-tile was waited for)
-                    publish_a();
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                    bar_named(1 + c.g, 128);
                 } else {
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    asm volatile("bar.sync 1, %0;" ::"n"(PF_ACT_WARPS * 32) : "memory");
-                    for (int c = t; c < Ly.N; c += PF_ACT_WARPS * 32) {
-                        const float m = fmaxf(fmaxf(pool_s[c], pool_s[256 + c]), fmaxf(pool_s[512 + c], pool_s[768 + c]));
-                        p.pooled[b * p.ldp + c] = m;
+                    bar_named(3, PF_ACT_WARPS * 32);
+                    for (int col = t; col < Ly.N; col += PF_ACT_WARPS * 32) {
+                        float m = pool_s[col];
+#pragma unroll
+                        for (int w = 1; w < PF_ACT_WARPS; ++w) m = fmaxf(m, pool_s[w * 256 + col]);
+                        p.pooled[b * p.ldp + col] = m;
                     }
-                    asm volatile("bar.sync 1, %0;" ::"n"(PF_ACT_WARPS * 32) : "memory");
+                    bar_named(3, PF_ACT_WARPS * 32);
                 }
             }
         }
-    }
-
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TM_COLS) : "memory");
-    }
-}
-
-// ------------------------------------------------------------------ bf16 variant (configs[3] arithmetic)
-// Same trunk with bf16 operands and fp32 accumulation: tcgen05.mma kind::f16, ONE MMA per product.
-// Activations travel between layers as bf16 in shared memory (K-major SWIZZLE_128B, 64 elements per
-// 128-byte row, written by the thread that owns the row); the weight image is bf16 (a quarter of the
-// 3xTF32 stream), 8-stage TMA ring.  Inputs and every layer output are rounded to bf16 (8-bit mantissa):
-// results agree with the fp32 path to ~1e-2 (tests state the bound), not to 1e-4.
-constexpr int PB_KC = 64;                                   // bf16 elements per K chunk (128-byte row)
-constexpr int PB_STAGES = 8;
-constexpr int PB_STAGE_BYTES = PF_NT * 128;                 // one (N-tile, K-chunk) weight block = 16 KB
-constexpr int PB_A_CHUNK_BYTES = PF_ROWS * 128;             // 16 KB
-constexpr int PB_A_BYTES = (PF_MAXK / PB_KC) * PB_A_CHUNK_BYTES;  // 32 KB
-
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-    // c = F32 (1 << 4), a = b = BF16 (1 << 7, 1 << 10), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ uint32_t pack_bf16x2(float e0, float e1) {  // e0 -> low half (lower address)
-    uint32_t r;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(e1), "f"(e0));
-    return r;
-}
-
-__global__ void __launch_bounds__(PF_THREADS, 1)
-pointnet_fused_bf16_kernel(const PfArgs p, const __grid_constant__ CUtensorMap wmap,
-                           const __grid_constant__ CUtensorMap xmap) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    if ((smem_u32(smem) & 1023u) != 0u) __trap();
-    // [A operand 32 KB][weight ring 8 x 16 KB][input tiles 2 x 8 KB][bias][pool scratch]
-    uint8_t* a_s = smem;
-    uint8_t* w_s = a_s + PB_A_BYTES;
-    uint8_t* x_s = w_s + PB_STAGES * PB_STAGE_BYTES;
-    float* bias_s = reinterpret_cast<float*>(x_s + 2 * PF_X_BYTES);
-    float* pool_s = bias_s + PF_MAX_BIAS;
-    __shared__ __align__(8) uint64_t bars[2 * PB_STAGES + 4 + 1 + PF_MAX_TILES];
-    __shared__ uint32_t tmem_base_s;
-    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
-    const uint32_t bars_u = smem_u32(&bars[0]);
-    auto w_full = [&](int s) { return bars_u + 8u * (uint32_t)s; };
-    auto w_empty = [&](int s) { return bars_u + 8u * (uint32_t)(PB_STAGES + s); };
-    auto x_full = [&](int s) { return bars_u + 8u * (uint32_t)(2 * PB_STAGES + s); };
-    auto x_empty = [&](int s) { return bars_u + 8u * (uint32_t)(2 * PB_STAGES + 2 + s); };
-    const uint32_t a_ready = bars_u + 8u * (2 * PB_STAGES + 4);
-    auto acc_full = [&](int nt) { return bars_u + 8u * (uint32_t)(2 * PB_STAGES + 5 + nt); };
-    if (t == 0) {
-        for (int s = 0; s < PB_STAGES; ++s) {
-            mbar_init(w_full(s), 1);
-            mbar_init(w_empty(s), 1);
-        }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(x_full(s), 1);
-            mbar_init(x_empty(s), PF_ACT_WARPS);
-        }
-        for (int s = 0; s < PF_MAX_TILES; ++s) mbar_init(acc_full(s), 1);
-        mbar_init(a_ready, PF_ACT_WARPS);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                         smem_u32(&tmem_base_s)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    SPG_PDL_ENTRY();  // set-up above overlaps the previous kernel of the stream; global memory only below
-    for (int i = t; i < p.n_bias; i += PF_THREADS) bias_s[i] = p.bias[i];
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
-    const uint32_t a_u = smem_u32(a_s), w_u = smem_u32(w_s), x_u = smem_u32(x_s);
-
-    if (warp == PF_ACT_WARPS) {
-        if (lane == 0) {  // ---- TMA producer
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&xmap) : "memory");
-            uint32_t it = 0, ci = 0;
-            for (int64_t b = blockIdx.x; b < p.B; b += gridDim.x, ++ci) {
-                const int xb = ci & 1;
-                mbar_wait(x_empty(xb), ((ci >> 1) & 1) ^ 1);
-                pf_expect_tx(x_full(xb), (uint32_t)(p.F * PF_ROWS * 4));
-                pf_tma_2d(x_u + xb * PF_X_BYTES, &xmap, 0, (int)(b * p.F), x_full(xb));
-                for (int l = 0; l < p.n_layers; ++l) {
-                    const PfLayer& Ly = p.L[l];
-                    const int ntile = Ly.N < PF_NT ? Ly.N : PF_NT;
-                    for (int nt = 0; nt < Ly.N / ntile; ++nt)
-                        for (int kc = 0; kc < Ly.K / PB_KC; ++kc, ++it) {
-                            const int s = it % PB_STAGES;
-                            mbar_wait(w_empty(s), ((it / PB_STAGES) & 1) ^ 1);
-                            pf_expect_tx(w_full(s), (uint32_t)(ntile * 128));
-                            // image rows of this layer: [kc*N + n], 128 bytes each; boxes of 32 rows
-                            for (int sub = 0; sub < ntile / 32; ++sub)
-                                pf_tma_2d(w_u + (uint32_t)(s * PB_STAGE_BYTES + sub * 32 * 128), &wmap, 0,
-                                          Ly.w_row + kc * Ly.N + nt * ntile + sub * 32, w_full(s));
-                        }
-                }
-            }
-        }
-    } else if (warp == PF_ACT_WARPS + 1) {
-        if (lane == 0) {  // ---- MMA issuer
-            uint32_t it = 0, q = 0;
-            for (int64_t b = blockIdx.x; b < p.B; b += gridDim.x) {
-                for (int l = 0; l < p.n_layers; ++l, ++q) {
-                    const PfLayer& Ly = p.L[l];
-                    const int ntile = Ly.N < PF_NT ? Ly.N : PF_NT;
-                    const uint32_t idesc = umma_idesc_bf16(PF_ROWS, ntile);
-                    mbar_wait(a_ready, q & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    for (int nt = 0; nt < Ly.N / ntile; ++nt) {
-                        const uint32_t d = tmem_base + (uint32_t)(nt * PF_NT);
-                        for (int kc = 0; kc < Ly.K / PB_KC; ++kc, ++it) {
-                            const int s = it % PB_STAGES;
-                            mbar_wait(w_full(s), (it / PB_STAGES) & 1);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                            const uint32_t a0 = a_u + (uint32_t)kc * PB_A_CHUNK_BYTES;
-                            const uint32_t b0 = w_u + (uint32_t)s * PB_STAGE_BYTES;
-#pragma unroll
-                            for (int ks = 0; ks < PB_KC / 16; ++ks)  // K = 16 bf16 = 32 bytes per instruction
-                                umma_bf16(d, umma_desc_k_sw128(a0 + ks * 32), umma_desc_k_sw128(b0 + ks * 32), idesc,
-                                          (kc | ks) ? 1u : 0u);
-                            umma_commit(w_empty(s));
-                        }
-                        umma_commit(acc_full(nt));
-                    }
-                }
-            }
-        }
-    } else {
-        // ---- activation warps: one thread per (point, half of the 32-column blocks)
-        const int quarter = warp & 3, half = warp >> 2;
-        const int row = quarter * 32 + lane;
-        const uint32_t lane_base = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        // 32 consecutive channels starting at channel col0 of the next A operand: 4 x 16 bytes of packed bf16
-        auto store_block = [&](int col0, const float (&o)[32]) {
-            const uint32_t base = a_u + (uint32_t)(col0 / PB_KC) * PB_A_CHUNK_BYTES;
-            const int c16_0 = (col0 % PB_KC) / 8;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const uint32_t q0 = pack_bf16x2(o[8 * j], o[8 * j + 1]), q1 = pack_bf16x2(o[8 * j + 2], o[8 * j + 3]);
-                const uint32_t q2 = pack_bf16x2(o[8 * j + 4], o[8 * j + 5]), q3 = pack_bf16x2(o[8 * j + 6], o[8 * j + 7]);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(base + sw128_off(row, c16_0 + j)),
-                             "r"(q0), "r"(q1), "r"(q2), "r"(q3) : "memory");
-            }
-        };
-        auto publish_a = [&]() {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) pf_arrive(a_ready);
-        };
-        const float zeros[32] = {0.f};
-        uint32_t ci = 0, acc_cnt[PF_MAX_TILES] = {0u, 0u};
-        for (int64_t b = blockIdx.x; b < p.B; b += gridDim.x, ++ci) {
-            const int xb = ci & 1;
-            mbar_wait(x_full(xb), (ci >> 1) & 1);
-            const float* xin = reinterpret_cast<const float*>(x_s + xb * PF_X_BYTES);
-            float v[32];
-#pragma unroll
-            for (int f = 0; f < 32; ++f) v[f] = (f < PF_MAXF && f < p.F) ? xin[f * PF_ROWS + row] : 0.f;
-            __syncwarp();
-            if (lane == 0) pf_arrive(x_empty(xb));
-            if (p.T && p.F >= 2) {
-                const float eye = p.add_eye ? 1.f : 0.f;
-                const float t00 = p.T[b * 4 + 0] + eye, t01 = p.T[b * 4 + 1], t10 = p.T[b * 4 + 2],
-                            t11 = p.T[b * 4 + 3] + eye;
-                const float x0 = v[0], x1 = v[1];
-                v[0] = fmaf(x0, t00, x1 * t10);
-                v[1] = fmaf(x0, t01, x1 * t11);
-            }
-            if (half == 0) store_block(0, v); else store_block(32, zeros);  // chunk 0: features | zero padding
-            publish_a();
-            for (int l = 0; l < p.n_layers; ++l) {
-                const PfLayer& Ly = p.L[l];
-                const int ntile = Ly.N < PF_NT ? Ly.N : PF_NT;
-                const bool last = l + 1 == p.n_layers;
-                for (int nt = 0; nt < Ly.N / ntile; ++nt) {
-                    mbar_wait(acc_full(nt), acc_cnt[nt] & 1);
-                    ++acc_cnt[nt];
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    for (int cb = half; cb < ntile / 32; cb += PF_ACT_WARPS / 4) {
-                        uint32_t r[32];
-                        tmem_ld32(lane_base + (uint32_t)(nt * PF_NT + cb * 32), r);
-                        const int col0 = nt * ntile + cb * 32;
-                        const float* bs = bias_s + Ly.b_off + col0;
-                        if (!last) {
-                            float o[32];
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) o[j] = fmaxf(__uint_as_float(r[j]) + bs[j], 0.f);
-                            store_block(col0, o);
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) {
-                                const float o = fmaxf(__uint_as_float(r[j]) + bs[j], 0.f);
-                                const unsigned m = __reduce_max_sync(0xffffffffu, __float_as_uint(o));
-                                if (lane == j) pool_s[quarter * 256 + col0 + j] = __uint_as_float(m);
-                            }
-                        }
-                    }
-                    // a 32-wide layer fills only half of the next 64-element K chunk: zero the other half
-                    if (!last && Ly.N == 32 && half == 1) store_block(32, zeros);
-                }
-                if (!last) {
-                    publish_a();
-                } else {
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    asm volatile("bar.sync 1, %0;" ::"n"(PF_ACT_WARPS * 32) : "memory");
-                    for (int c = t; c < Ly.N; c += PF_ACT_WARPS * 32) {
-                        const float m = fmaxf(fmaxf(pool_s[c], pool_s[256 + c]), fmaxf(pool_s[512 + c], pool_s[768 + c]));
-                        p.pooled[b * p.ldp + c] = m;
-                    }
-                    asm volatile("bar.sync 1, %0;" ::"n"(PF_ACT_WARPS * 32) : "memory");
-                }
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
     }
 }
 
@@ -651,10 +465,10 @@ int spg_pointnet_fused_eval(const float* clouds, int64_t n_clouds, int n_feature
     rc = pf_map_2d(&xmap, clouds, PF_ROWS, (uint64_t)(n_clouds * n_features), PF_ROWS, (uint32_t)n_features);
     if (rc) return rc;
     const int64_t grid = n_clouds < kNumSMs ? n_clouds : kNumSMs;
-    const int smem = PF_STAGES_TMEM_A * PF_STAGE_BYTES + 2 * PF_X_BYTES + (PF_MAX_BIAS + 4 * 256) * 4;
-    cudaError_t e = cudaFuncSetAttribute(pointnet_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    const int smem = PfCfg<false>::SMEM;
+    cudaError_t e = cudaFuncSetAttribute(pointnet_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return (int)e;
-    SPG_LAUNCH(K_POINTNET_FUSED, (cudaStream_t)stream, pointnet_fused_kernel, (unsigned)grid, PF_THREADS, smem,
+    SPG_LAUNCH(K_POINTNET_FUSED, (cudaStream_t)stream, pointnet_fused_kernel<false>, (unsigned)grid, PF_THREADS, smem,
                a, wmap, xmap);
     return launch_status();
 }
@@ -710,10 +524,10 @@ int spg_pointnet_fused_eval_bf16(const float* clouds, int64_t n_clouds, int n_fe
     rc = pf_map_2d(&xmap, clouds, PF_ROWS, (uint64_t)(n_clouds * n_features), PF_ROWS, (uint32_t)n_features);
     if (rc) return rc;
     const int64_t grid = n_clouds < kNumSMs ? n_clouds : kNumSMs;
-    const int smem = PB_A_BYTES + PB_STAGES * PB_STAGE_BYTES + 2 * PF_X_BYTES + (PF_MAX_BIAS + 4 * 256) * 4;
-    cudaError_t e = cudaFuncSetAttribute(pointnet_fused_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    const int smem = PfCfg<true>::SMEM;
+    cudaError_t e = cudaFuncSetAttribute(pointnet_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return (int)e;
-    SPG_LAUNCH(K_POINTNET_FUSED, (cudaStream_t)stream, pointnet_fused_bf16_kernel, (unsigned)grid, PF_THREADS, smem, a,
+    SPG_LAUNCH(K_POINTNET_FUSED, (cudaStream_t)stream, pointnet_fused_kernel<true>, (unsigned)grid, PF_THREADS, smem, a,
                wmap, xmap);
     return launch_status();
 }

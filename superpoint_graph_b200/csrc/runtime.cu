@@ -50,7 +50,7 @@ static cudaEvent_t get_event() {
 static std::atomic<int> g_pdl{-1};  // -1: read SPG_PDL from the environment on first use (default on)
 
 // mode 0: off; 1: every kernel; 2: every kernel except the persistent tensor-core kernels; 3: only the
-// tcgen05 GEMM and its merge companion
+// tensor-core GEMM and its merge companion
 bool pdl_enabled(int kid) {
     int v = g_pdl.load(std::memory_order_relaxed);
     if (v < 0) {

@@ -1,15 +1,15 @@
-// tcgen05 weight-gradient GEMM of the point-wise layers:
+// Hopper (wgmma) weight-gradient GEMM of the point-wise layers:
 //
 //     dW[Co, Ci] = sum_m dY[m, Co] * f(P)[m, Ci]        (m runs over all Nv*L points)
 //
-// Both operands are read exactly as they lie in HBM (point-major rows, channels contiguous), i.e.
-// the reduction dimension is the OUTER one: for the tensor core this is an "MN-major x MN-major"
-// product, D[Co,Ci] += A[Co,k] * B[Ci,k]^T with k = points.  A CTA owns a contiguous slab of points,
-// streams it in chunks of 32 points through a 2-stage shared-memory ring (MN-major SWIZZLE_128B
-// SW128_32B atoms: 32 channels x 4 points = 512 B), splits every value into tf32 hi/lo on the fly (3xTF32,
-// fp32-equivalent), keeps the full [Co,Ci] accumulator in TMEM (Co/128 tiles x Ci columns) for
-// its whole lifetime and finally writes one partial per CTA; gemm_splitk_reduce adds the partials
-// in a fixed order (deterministic).  f = affine + ReLU of the layer that produced P (fused).
+// Both operands lie in HBM point-major (channels contiguous), i.e. the reduction dimension is the OUTER
+// one.  wgmma reads tf32 operands K-major only, so the CTA transposes while it stages: it owns a
+// contiguous slab of points, streams it in chunks of 32 points (one 128-byte SWIZZLE_128B row per
+// channel) through a 2-stage shared-memory ring, splitting every value into tf32 hi/lo on the fly (3xTF32,
+// fp32-equivalent).  Two warpgroups keep the [Co, Ci] accumulator in registers for the CTA's whole
+// lifetime (Co >= 128: half of the rows each; Co = 64: half of the columns each) and finally write one
+// partial per CTA; gemm_splitk_reduce adds the partials in a fixed order (deterministic).
+// f = affine + ReLU of the layer that produced P (fused).
 //
 // Reference semantics: the weight gradient of nn.Conv1d(k=1) (learning/pointnet.py:29,85) as
 // autograd computes it; the reference materialises ReLU(BN(P)) and runs cuDNN/cuBLAS on it.
@@ -19,7 +19,7 @@
 namespace spg {
 
 constexpr int DW_THREADS = 256;
-constexpr int DW_PTS = 32;  // points per chunk (4 UMMA K-steps of 8)
+constexpr int DW_PTS = 32;  // points per chunk (4 wgmma K-steps of 8)
 
 struct DwArgs {
     const float* dY;
@@ -33,102 +33,79 @@ struct DwArgs {
     int64_t pts_per_cta;  // multiple of DW_PTS
 };
 
-// byte offset of (point pt in [0,32), 16-byte channel chunk c4) in an MN-major SW128_32B tile with
-// MB 32-channel blocks: 512-byte atoms (32 channels x 4 points) ordered [point group][channel block];
-// inside an atom the 32-byte chunk index is XORed with the point row (Swizzle<2,5,2>).
-template <int MB>
-__device__ __forceinline__ uint32_t mn_off(int pt, int c4) {
-    const int kg = pt >> 2, kr = pt & 3, mb = c4 >> 3, j = c4 & 7;
-    return (uint32_t)((kg * MB + mb) * 512 + kr * 128 + (((j >> 1) ^ kr) << 5) + ((j & 1) << 4));
-}
-
 template <int CO, int CI>
 __global__ void __launch_bounds__(DW_THREADS, 1) tc_dw_kernel(const DwArgs p) {
-    constexpr int CO_PAD = CO < 128 ? 128 : CO;  // the accumulator tile has 128 rows (UMMA M)
-    constexpr int MB_A = CO_PAD / 32, MB_B = CI / 32;
-    constexpr int A_BYTES = CO_PAD * DW_PTS * 4;  // one of hi|lo
+    constexpr int WM = CO >= 128 ? CO / 2 : 64;  // accumulator rows of one warpgroup
+    constexpr int WN = CO >= 128 ? CI : CI / 2;  // accumulator columns of one warpgroup
+    constexpr int MSUB = WM / 64;                 // m64 sub-tiles
+    constexpr int A_BYTES = CO * DW_PTS * 4;      // one of hi|lo: [CO rows][128 B]
     constexpr int B_BYTES = CI * DW_PTS * 4;
     constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-    constexpr int MT = CO_PAD / 128;              // 128-row accumulator tiles
-    constexpr int TMEM_COLS_RAW = MT * CI;
-    constexpr int TMEM_COLS = TMEM_COLS_RAW <= 32 ? 32 : TMEM_COLS_RAW <= 64 ? 64 : TMEM_COLS_RAW <= 128 ? 128 : TMEM_COLS_RAW <= 256 ? 256 : 512;
-    static_assert(CO % 64 == 0 && CI % 32 == 0 && CI <= 256 && TMEM_COLS_RAW <= 512, "shape");
+    static_assert(CO % 64 == 0 && CI % 32 == 0 && CI <= 128 && CO <= 256, "shape");
     constexpr int A_F4 = CO * DW_PTS / 4 / DW_THREADS;  // float4 per thread per chunk
     constexpr int B_F4 = CI * DW_PTS / 4 / DW_THREADS;
 
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    __shared__ __align__(8) uint64_t bars[3];
-    __shared__ uint32_t tmem_base_s;
 
     const int t = threadIdx.x;
     const int warp = t >> 5, lane = t & 31;
-    const uint32_t bar_empty0 = smem_u32(&bars[0]), bar_empty1 = smem_u32(&bars[1]);
-    const uint32_t bar_done = smem_u32(&bars[2]);
-    if (t == 0) {
-        mbar_init(bar_empty0, 1);
-        mbar_init(bar_empty1, 1);
-        mbar_init(bar_done, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                         smem_u32(&tmem_base_s)),
-                     "r"((uint32_t)TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
-    if (CO < CO_PAD) {
-        // channels CO..127 of the A tiles are never written by the loads: zero them once
-        for (int i = t; i < 2 * STAGE_BYTES / 16; i += DW_THREADS)
-            reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
-        __syncthreads();
-    }
-    SPG_PDL_ENTRY();  // set-up above overlaps the previous kernel of the stream; global memory only below
+    const int g = warp >> 2, wl = warp & 3;
+    SPG_PDL_ENTRY();
 
     const int64_t m_beg = (int64_t)blockIdx.x * p.pts_per_cta;
     const int64_t m_end = min(p.M, m_beg + p.pts_per_cta);
     const int nchunks = m_beg < m_end ? (int)((m_end - m_beg + DW_PTS - 1) / DW_PTS) : 0;
-    constexpr uint32_t idesc = umma_idesc_tf32_major(128, CI, 1, 1);
     const bool pro = p.p_scale || p.p_shift || p.p_relu;
 
+    // Thread i of a chunk handles the float4 (point pt, channels 4*c4..4*c4+3): a warp covers 8 points x
+    // 4 channel groups, so that its 64-byte row segments are whole sectors and its transposed 4-byte
+    // shared-memory stores spread over 16 banks.
+    auto coord = [](int i, int c4s, int& pt, int& c4) {
+        const int wi = i >> 5, l = i & 31;
+        pt = (wi & 3) * 8 + (l & 7);
+        c4 = (wi >> 2) * 4 + (l >> 3);
+        (void)c4s;
+    };
     float4 ra[A_F4], rb[B_F4];
     auto load_chunk = [&](int ch) {
         const int64_t mrow = m_beg + (int64_t)ch * DW_PTS;
 #pragma unroll
         for (int j = 0; j < A_F4; ++j) {
-            const int i = t + DW_THREADS * j;
-            const int pt = i / (CO / 4), c4 = i % (CO / 4);
+            int pt, c4;
+            coord(t + DW_THREADS * j, CO / 4, pt, c4);
             ra[j] = (mrow + pt < m_end)
                         ? __ldg(reinterpret_cast<const float4*>(p.dY + (mrow + pt) * p.lddy + c4 * 4))
                         : make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
         for (int j = 0; j < B_F4; ++j) {
-            const int i = t + DW_THREADS * j;
-            const int pt = i / (CI / 4), c4 = i % (CI / 4);
+            int pt, c4;
+            coord(t + DW_THREADS * j, CI / 4, pt, c4);
             rb[j] = (mrow + pt < m_end)
                         ? __ldg(reinterpret_cast<const float4*>(p.P + (mrow + pt) * p.ldp + c4 * 4))
                         : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     };
-    auto split_store = [&](uint8_t* hi_base, uint8_t* lo_base, uint32_t off, float4 v) {
-        uint4 hi, lo;
-        hi.x = to_tf32(v.x);
-        hi.y = to_tf32(v.y);
-        hi.z = to_tf32(v.z);
-        hi.w = to_tf32(v.w);
-        lo.x = to_tf32(v.x - __uint_as_float(hi.x));
-        lo.y = to_tf32(v.y - __uint_as_float(hi.y));
-        lo.z = to_tf32(v.z - __uint_as_float(hi.z));
-        lo.w = to_tf32(v.w - __uint_as_float(hi.w));
-        *reinterpret_cast<uint4*>(hi_base + off) = hi;
-        *reinterpret_cast<uint4*>(lo_base + off) = lo;
+    // (point pt, channels 4*c4 + e) -> K-major row 4*c4 + e, element pt of its 128-byte row
+    auto split_store = [&](uint8_t* hi_base, uint8_t* lo_base, int pt, int c4, float4 v) {
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const uint32_t off = sw128_off(4 * c4 + e, pt >> 2) + (uint32_t)(pt & 3) * 4u;
+            const uint32_t hi = to_tf32(vv[e]);
+            *reinterpret_cast<uint32_t*>(hi_base + off) = hi;
+            *reinterpret_cast<uint32_t*>(lo_base + off) = to_tf32(vv[e] - __uint_as_float(hi));
+        }
     };
+
+    float acc[MSUB][WN / 2];
+#pragma unroll
+    for (int m = 0; m < MSUB; ++m)
+#pragma unroll
+        for (int i = 0; i < WN / 2; ++i) acc[m][i] = 0.f;
+    const int row_g = CO >= 128 ? g * WM : 0;  // first accumulator row / column of this warpgroup
+    const int col_g = CO >= 128 ? 0 : g * WN;
 
     if (nchunks > 0) load_chunk(0);
     for (int ch = 0; ch < nchunks; ++ch) {
@@ -138,18 +115,22 @@ __global__ void __launch_bounds__(DW_THREADS, 1) tc_dw_kernel(const DwArgs p) {
         uint8_t* a_lo = stage + A_BYTES;
         uint8_t* b_hi = stage + 2 * A_BYTES;
         uint8_t* b_lo = b_hi + B_BYTES;
-        if (ch >= 2) mbar_wait(s ? bar_empty1 : bar_empty0, (uint32_t)(((ch >> 1) - 1) & 1));
+        // the products of chunk ch-2 (the last reader of this stage) have completed in both warpgroups
+        wg_wait<1>();
+        wg_reg_fence(acc[0]);
+        if (MSUB > 1) wg_reg_fence(acc[MSUB - 1]);
+        __syncthreads();
         const int64_t mrow = m_beg + (int64_t)ch * DW_PTS;
 #pragma unroll
         for (int j = 0; j < A_F4; ++j) {
-            const int i = t + DW_THREADS * j;
-            const int pt = i / (CO / 4), c4 = i % (CO / 4);
-            split_store(a_hi, a_lo, mn_off<MB_A>(pt, c4), ra[j]);
+            int pt, c4;
+            coord(t + DW_THREADS * j, CO / 4, pt, c4);
+            split_store(a_hi, a_lo, pt, c4, ra[j]);
         }
 #pragma unroll
         for (int j = 0; j < B_F4; ++j) {
-            const int i = t + DW_THREADS * j;
-            const int pt = i / (CI / 4), c4 = i % (CI / 4);
+            int pt, c4;
+            coord(t + DW_THREADS * j, CI / 4, pt, c4);
             float4 v = rb[j];
             if (pro && (mrow + pt < m_end)) {
                 float4 sc = make_float4(1.f, 1.f, 1.f, 1.f), sh = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -166,79 +147,55 @@ __global__ void __launch_bounds__(DW_THREADS, 1) tc_dw_kernel(const DwArgs p) {
                     v.w = fmaxf(v.w, 0.f);
                 }
             }
-            split_store(b_hi, b_lo, mn_off<MB_B>(pt, c4), v);
+            split_store(b_hi, b_lo, pt, c4, v);
         }
-        if (ch + 1 < nchunks) load_chunk(ch + 1);  // in flight while the tensor core works
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
-        if (t == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t ah = smem_u32(a_hi), al = smem_u32(a_lo);
-            const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+        {
+            const uint32_t ah = smem_u32(a_hi) + (uint32_t)row_g * 128u, al = smem_u32(a_lo) + (uint32_t)row_g * 128u;
+            const uint32_t bh = smem_u32(b_hi) + (uint32_t)col_g * 128u, bl = smem_u32(b_lo) + (uint32_t)col_g * 128u;
+#pragma unroll
+            for (int m = 0; m < MSUB; ++m) wg_reg_fence(acc[m]);
+            wg_fence();
 #pragma unroll
             for (int kb = 0; kb < DW_PTS / 8; ++kb) {
-                // one K-step = 8 points = two 4-point groups (sbo apart)
-                const uint64_t dbh = umma_desc_mn_sw128_32b(bh + 2 * kb * MB_B * 512, 512, MB_B * 512);
-                const uint64_t dbl = umma_desc_mn_sw128_32b(bl + 2 * kb * MB_B * 512, 512, MB_B * 512);
+                const uint64_t dbh = wg_desc_k_sw128(bh + kb * 32), dbl = wg_desc_k_sw128(bl + kb * 32);
 #pragma unroll
-                for (int mt = 0; mt < MT; ++mt) {
-                    const uint32_t aoff = (2 * kb * MB_A + mt * 4) * 512;
-                    const uint64_t dah = umma_desc_mn_sw128_32b(ah + aoff, 512, MB_A * 512);
-                    const uint64_t dal = umma_desc_mn_sw128_32b(al + aoff, 512, MB_A * 512);
-                    const uint32_t d = tmem_base + mt * CI;
-                    umma_tf32(d, dah, dbh, idesc, (ch | kb) ? 1u : 0u);
-                    umma_tf32(d, dal, dbh, idesc, 1u);
-                    umma_tf32(d, dah, dbl, idesc, 1u);
+                for (int m = 0; m < MSUB; ++m) {
+                    const uint64_t dah = wg_desc_k_sw128(ah + m * 64 * 128 + kb * 32);
+                    const uint64_t dal = wg_desc_k_sw128(al + m * 64 * 128 + kb * 32);
+                    wgmma_tf32<WN>(acc[m], dah, dbh, 1u);
+                    wgmma_tf32<WN>(acc[m], dal, dbh, 1u);
+                    wgmma_tf32<WN>(acc[m], dah, dbl, 1u);
                 }
             }
-            umma_commit(s ? bar_empty1 : bar_empty0);
-            if (ch == nchunks - 1) umma_commit(bar_done);
+            wg_commit();
         }
+        if (ch + 1 < nchunks) load_chunk(ch + 1);  // in flight while the tensor core works
     }
+    wg_wait<0>();
+#pragma unroll
+    for (int m = 0; m < MSUB; ++m) wg_reg_fence(acc[m]);
 
-    // ---- epilogue: accumulator -> this CTA's partial [CO, CI]
+    // ---- epilogue: accumulator -> this CTA's partial [CO, CI] (zeros when the CTA got no points)
     float* out = p.partial + (int64_t)blockIdx.x * CO * CI;
-    if (nchunks > 0) {
-        mbar_wait(bar_done, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    {
-        const int q = warp & 3, half = warp >> 2;
-        constexpr int NBLK = CI / 32;  // 32-column blocks per accumulator tile
+    const int r = lane >> 2, cq = 2 * (lane & 3);
 #pragma unroll
-        for (int mt = 0; mt < MT; ++mt) {
-            const int row = mt * 128 + q * 32 + lane;
-            if (row >= CO) continue;  // padded accumulator rows
-            for (int cb = half; cb < NBLK; cb += 2) {
-                float4* dst = reinterpret_cast<float4*>(out + (int64_t)row * CI + cb * 32);
-                if (nchunks > 0) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mt * CI + cb * 32), r);
+    for (int m = 0; m < MSUB; ++m) {
+        const int row = row_g + m * 64 + wl * 16 + r;
 #pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]),
-                                             __uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3]));
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) dst[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-            }
+        for (int j = 0; j < WN / 8; ++j) {
+            const int col = col_g + 8 * j + cq;
+            *reinterpret_cast<float2*>(out + (int64_t)row * CI + col) = make_float2(acc[m][4 * j], acc[m][4 * j + 1]);
+            *reinterpret_cast<float2*>(out + (int64_t)(row + 8) * CI + col) =
+                make_float2(acc[m][4 * j + 2], acc[m][4 * j + 3]);
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                     "r"((uint32_t)TMEM_COLS)
-                     : "memory");
     }
 }
 
 template <int CO, int CI>
 static int launch_dw(const DwArgs& a, int ctas, cudaStream_t s) {
-    constexpr int CO_PAD = CO < 128 ? 128 : CO;
-    constexpr int STAGE_BYTES = 2 * CO_PAD * DW_PTS * 4 + 2 * CI * DW_PTS * 4;
+    constexpr int STAGE_BYTES = 2 * CO * DW_PTS * 4 + 2 * CI * DW_PTS * 4;
     const int smem = 2 * STAGE_BYTES + 1024;
     cudaError_t e = cudaFuncSetAttribute(tc_dw_kernel<CO, CI>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return (int)e;

@@ -1,43 +1,32 @@
-// tcgen05 3xTF32 GEMM for the point-wise layers: persistent, warp-specialised, weights resident in
-// SMEM (loaded by TMA), with the BatchNorm bookkeeping of the training step fused on both sides.
+// Hopper (wgmma) 3xTF32 GEMM for the point-wise layers: persistent, warp-specialised, weights resident
+// in SMEM (loaded by TMA), with the BatchNorm bookkeeping of the training step fused on both sides.
 //
 //     C[M,N] = f(A)[M,K] * B[N,K]^T + bias
 //
 // in fp32-equivalent precision through error-compensated 3xTF32 splitting
 // (x = hi + lo with hi = tf32(x), lo = tf32(x - hi);  A*B ~= Ahi*Bhi + Alo*Bhi + Ahi*Blo, all three
-// accumulated in the same fp32 TMEM accumulator; single-pass TF32 cannot hold the 1e-4 parity bound
+// accumulated in the same fp32 register accumulator; single-pass TF32 cannot hold the 1e-4 parity bound
 // through five layers + BatchNorm, 3xTF32 is at ~1e-6).
 //
 // A CTA (one per SM) owns an N-slice of NS <= 128 output channels whose pre-split weight image
 // (hi+lo, <= 128 KB) is brought into shared memory ONCE by cp.async.bulk.tensor (TMA, one 2-D box
-// per (K-chunk, hi|lo) block of the image, completion on an mbarrier), and then walks over row tiles:
+// per (K-chunk, hi|lo) block of the image, completion on an mbarrier), and then walks over 128-row tiles:
 //
-//   warps 0-3   epilogue : tcgen05.ld accumulator -> +bias -> per-warp transpose tile -> 128-byte
-//                          line stores, plus ONE of the fused column reductions
-//                            STATS : batch statistics of C (pivoted sums kept per CTA across tiles)
-//                            BNRED : BatchNorm-backward sums of the layer BELOW (C is its dL/d(act)):
-//                                    s1 = sum gz, s2 = sum gz*xhat with gz = relu'(y2) * C
-//   warp  4     MMA      : one thread issues 12 tcgen05.mma per K-chunk, tcgen05.commit -> mbarriers
-//   warps 5-12  producer : coalesced 128-bit loads of A (next chunks prefetched in registers), fused
-//                          prologue, tf32 hi/lo split, SWIZZLE_128B K-major tiles, 2..4-stage ring
-//                            AFFINE : f = relu(a*scale + shift)          (forward: BN apply + ReLU)
-//                            BNBWD  : f = scale*(gz - s1/M - xhat*s2/M)  (backward: A = dL/d(act),
-//                                     A2 = raw output y of the layer; optional side store of f)
+//   warps 0-7   consumers: two warpgroups, each issues wgmma.mma_async m64 x NS x k8 over its 64 rows of
+//               the tile (12 per K chunk), then runs the epilogue straight from the register accumulator:
+//               +bias -> C, plus ONE of the fused column reductions
+//                 STATS : batch statistics of C (pivoted sums kept per warp across tiles)
+//                 BNRED : BatchNorm-backward sums of the layer BELOW (C is its dL/d(act)):
+//                         s1 = sum gz, s2 = sum gz*xhat with gz = relu'(y2) * C
+//   warps 8-15  producers: coalesced 128-bit loads of A (next chunks prefetched in registers), fused
+//               prologue, tf32 hi/lo split, SWIZZLE_128B K-major tiles, 2..4-stage ring
+//                 AFFINE : f = relu(a*scale + shift)          (forward: BN apply + ReLU)
+//                 BNBWD  : f = scale*(gz - s1/M - xhat*s2/M)  (backward: A = dL/d(act),
+//                          A2 = raw output y of the layer; optional side store of f)
 //
 // The column reductions leave ONE partial per CTA and column (pivoted sums are carried across the
-// CTA's tiles); a 32-block companion kernel (tc_merge_kernel, same C-ABI call) folds the <= 148
-// partials per column in a fixed order (deterministic) into mean/var/scale/shift/running statistics
-// or s1/s2.  Round 1 wrote a partial per (tile, warp) — 3768 per column — and needed a two-level
-// merge plus separate BatchNorm-backward reduce/apply passes (0.85 of 1.95 ms per step).
-//
-// Measured limits (profiles/README.md, round 2): in steady state (1.29 M rows) the forward variant holds the
-// tensor pipe 35 % busy while the shared-memory data pipe is ~80 % busy (LSU 45 % + tensor-core operand
-// reads 34 %): 3xTF32 reads A and B twice per K chunk on top of the producers' 32 KB of stores per chunk.
-// Tried and rejected (each measured slower or equal): an A-operand ring in tensor memory written by
-// thread-per-row producers (uncoalesced 64-byte row segments: 585 -> 675 us at 1.29 M rows), L2 prefetch of
-// the rows 10 chunks ahead, a 3-deep register ring for the two-operand prologue (spills at the 128-register
-// cap of a 13-warp CTA), an in-kernel grid barrier for the merge (cooperative launch serialises against the
-// side stream).
+// CTA's tiles); a companion kernel (tc_merge_kernel, same C-ABI call) folds the <= kNumSMs partials per
+// column in a fixed order (deterministic) into mean/var/scale/shift/running statistics or s1/s2.
 //
 // Reference semantics: nn.Conv1d(k=1)+BatchNorm1d+ReLU stacks of learning/pointnet.py:27-37,83-96
 // and their autograd backward.
@@ -54,11 +43,10 @@ namespace spg {
 constexpr int T2_BM = 128;
 constexpr int T2_KC = 32;
 constexpr int T2_MAX_STAGES = 4;  // the A ring gets as many stages as fit next to the resident weights
-constexpr int T2_EPI_WARPS = 4, T2_PROD_WARPS = 8;  // (8 epilogue warps force 96 regs/thread: measured slower)
-constexpr int T2_THREADS = (T2_EPI_WARPS + 1 + T2_PROD_WARPS) * 32;  // 416
-constexpr int T2_A_BYTES = T2_BM * T2_KC * 4;                        // 16 KB (hi or lo)
+constexpr int T2_EPI_WARPS = 8, T2_PROD_WARPS = 8;  // consumers: two warpgroups of 64 rows each
+constexpr int T2_THREADS = (T2_EPI_WARPS + T2_PROD_WARPS) * 32;  // 512
+constexpr int T2_A_BYTES = T2_BM * T2_KC * 4;                    // 16 KB (hi or lo)
 constexpr int T2_STAGE_BYTES = 2 * T2_A_BYTES;
-constexpr int T2_EPI_PITCH = 36;  // floats per row of an epilogue transpose tile (16-byte aligned rows)
 
 enum { PRO_AFFINE = 0, PRO_BNBWD = 1 };
 enum { EPI_NONE = 0, EPI_STATS = 1, EPI_BNRED = 2 };
@@ -98,14 +86,6 @@ struct Tc2Args {
     int nstages;   // A-ring depth (2..4)
 };
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-
 // 2-D TMA load global -> shared, completion counted on an mbarrier (coordinates: {x = innermost, y})
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
     asm volatile(
@@ -122,8 +102,7 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     // it): SWIZZLE_128B atoms need that, and no spare bytes are reserved for a manual round-up
     uint8_t* smem = smem_raw;
     if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
-    __shared__ __align__(8) uint64_t bars[2 * T2_MAX_STAGES + 5];
-    __shared__ uint32_t tmem_base_s;
+    __shared__ __align__(8) uint64_t bars[2 * T2_MAX_STAGES + 1];
 
     const int t = threadIdx.x;
     const int warp = t >> 5, lane = t & 31;
@@ -136,34 +115,20 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     const uint32_t bars_u32 = smem_u32(&bars[0]);
     auto bar_full = [&](int s) { return bars_u32 + 8u * (uint32_t)s; };
     auto bar_empty = [&](int s) { return bars_u32 + 8u * (uint32_t)(T2_MAX_STAGES + s); };
-    auto bar_accfull = [&](uint32_t a) { return bars_u32 + 8u * (2 * T2_MAX_STAGES + a); };
-    auto bar_accempty = [&](uint32_t a) { return bars_u32 + 8u * (2 * T2_MAX_STAGES + 2 + a); };
-    const uint32_t bar_w = bars_u32 + 8u * (2 * T2_MAX_STAGES + 4);
+    const uint32_t bar_w = bars_u32 + 8u * (2 * T2_MAX_STAGES);
 
     if (t == 0) {
 #pragma unroll
         for (int s = 0; s < T2_MAX_STAGES; ++s) {
             mbar_init(bar_full(s), T2_PROD_WARPS);  // one elected arrival per producer warp
-            mbar_init(bar_empty(s), 1);
+            mbar_init(bar_empty(s), T2_EPI_WARPS);  // one elected arrival per consumer warp
         }
-        mbar_init(bar_accfull(0), 1);
-        mbar_init(bar_accfull(1), 1);
-        mbar_init(bar_accempty(0), T2_EPI_WARPS);  // one elected arrival per epilogue warp
-        mbar_init(bar_accempty(1), T2_EPI_WARPS);
         mbar_init(bar_w, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
     }
-    if (warp == 0) {
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                         smem_u32(&tmem_base_s)),
-                     "r"((uint32_t)(2 * NS < 32 ? 32 : 2 * NS))
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // Everything above (barrier init, descriptor prefetch, tensor-memory allocation) overlaps the previous
-    // kernel of the stream; nothing below this line runs before that kernel's results are visible.
+    // Everything above (barrier init, descriptor prefetch) overlaps the previous kernel of the stream;
+    // nothing below this line runs before that kernel's results are visible.
     SPG_PDL_ENTRY();
     if (t == 0) {
         // resident weight slice by TMA: rows [n0, n0+NS) of every (chunk, hi|lo) block of the image
@@ -176,12 +141,12 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     // Producer threads put their first A chunks in flight before anything else: the global-load
     // latency then overlaps the resident-weight load and the CTA-wide barrier below.
     // Register-level prefetch ring: PF chunks of A are in flight per thread (the global-load
-    // latency, ~2 us under load, is far longer than one chunk's transform + MMA).  The BNBWD
+    // latency under load is far longer than one chunk's transform + MMA).  The BNBWD
     // prologue streams two operands, so its ring is half as deep (same register budget).
-    constexpr int PF = PRO == PRO_BNBWD ? 2 : 4;  // (3 spills at the 128-register cap of a 13-warp CTA)
+    constexpr int PF = PRO == PRO_BNBWD ? 2 : 4;
     constexpr int NOPS = PRO == PRO_BNBWD ? 2 : 1;
     float4 q[PF][NOPS][4];
-    const int pt = t - (T2_EPI_WARPS + 1) * 32;  // producer thread id 0..255 (negative: other roles)
+    const int pt = t - T2_EPI_WARPS * 32;  // producer thread id 0..255 (negative: consumers)
     auto load = [&](int64_t tile, int kc, float4 (&dst)[NOPS][4]) {
         const int64_t m0 = tile * T2_BM;
 #pragma unroll
@@ -220,10 +185,7 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     float* c0_s = cy_s + p.K;   // BNBWD: constant term
     float* bias_s = c0_s + p.K;
     float* ev_s = bias_s + NS;  // BNRED: [4][NS] = scale2, shift2, mean2, rstd2 of the layer below
-    float* acc_s = ev_s + 4 * NS;  // column accumulators [4 epilogue warps][NS][4]
-    // per-epilogue-warp transpose tiles [32 rows][36]: accumulator rows (one per lane) are turned
-    // into full 128-byte lines before they go to global memory
-    float* epi_s = acc_s + T2_EPI_WARPS * NS * 4;
+    float* acc_s = ev_s + 4 * NS;  // column accumulators [8 consumer warps][NS][4]
     for (int i = t; i < p.K; i += T2_THREADS) {
         const float sc = p.a_scale ? p.a_scale[i] : 1.f;
         sc_s[i] = sc;
@@ -246,13 +208,9 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
         }
     }
     for (int i = t; i < T2_EPI_WARPS * NS * 4; i += T2_THREADS) acc_s[i] = 0.f;
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_s;
 
-    if (warp >= T2_EPI_WARPS + 1) {
+    if (warp >= T2_EPI_WARPS) {
         // ================================ producers ================================
         const bool pro = PRO == PRO_BNBWD || p.a_scale || p.a_shift || p.a_relu;
         int64_t tile = blockIdx.x;
@@ -342,172 +300,129 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
                 if (tile >= tiles) break;
             }
         }
-    } else if (warp == T2_EPI_WARPS) {
-        // ================================ MMA issuer ================================
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_tf32(T2_BM, NS);
-            const uint32_t wres_u32 = smem_u32(wres);
-            uint32_t it = 0, tcount = 0;
-            mbar_wait(bar_w, 0);  // resident weights have landed (TMA complete_tx)
-            for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tcount) {
-                const uint32_t a = tcount & 1;
-                if (tcount >= 2) mbar_wait(bar_accempty(a), ((tcount >> 1) - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t d = tmem_base + a * NS;
-                for (int kc = 0; kc < nk; ++kc, ++it) {
-                    const int s = it % nst;
-                    mbar_wait(bar_full(s), (it / nst) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t a_hi = smem_u32(smem + (size_t)s * T2_STAGE_BYTES);
-                    const uint32_t a_lo = a_hi + T2_A_BYTES;
-                    const uint32_t b_hi = wres_u32 + (uint32_t)(kc * 2) * (NS * T2_KC * 4);
-                    const uint32_t b_lo = b_hi + NS * T2_KC * 4;
-#pragma unroll
-                    for (int ks = 0; ks < T2_KC / 8; ++ks) {
-                        const uint32_t ko = ks * 32;
-                        const uint64_t dah = umma_desc_k_sw128(a_hi + ko), dal = umma_desc_k_sw128(a_lo + ko);
-                        const uint64_t dbh = umma_desc_k_sw128(b_hi + ko), dbl = umma_desc_k_sw128(b_lo + ko);
-                        umma_tf32(d, dah, dbh, idesc, (kc | ks) ? 1u : 0u);
-                        umma_tf32(d, dal, dbh, idesc, 1u);
-                        umma_tf32(d, dah, dbl, idesc, 1u);
-                    }
-                    umma_commit(bar_empty(s));
-                }
-                umma_commit(bar_accfull(a));
-            }
-        }
     } else {
-        // ================================ epilogue ================================
-        const int w = warp & 3;      // TMEM lane quarter this warp may access
-        uint32_t tcount = 0;
+        // ======================= consumers: wgmma + epilogue from registers =======================
+        const int g = warp >> 2, wl = warp & 3;  // warpgroup (64-row half of the tile), warp in it
+        const int r = lane >> 2, cq = 2 * (lane & 3);
         float* acc_w = acc_s + warp * (NS * 4);
-        float* tile_s = epi_s + warp * (32 * T2_EPI_PITCH);
-        for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++tcount) {
-            const uint32_t a = tcount & 1;
-            mbar_wait(bar_accfull(a), (tcount >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int64_t row0 = tile * T2_BM + w * 32;
-            const int nv = (int)max((int64_t)0, min((int64_t)32, p.M - row0));
-#pragma unroll 1
-            for (int cb = 0; cb < NS / 32; ++cb) {
-                const int col0 = n0 + cb * 32;
-                const int rr = lane >> 3, c4 = lane & 7;
-                // BNRED: the y rows of the layer below are put in flight before the accumulator is
-                // read, so that their global-load latency hides behind tcgen05.ld + the transpose
-                float4 yv[8];
-                if (p.epi == EPI_BNRED) {
+        const uint32_t wres_u32 = smem_u32(wres);
+        const uint32_t smem_u = smem_u32(smem);
+        float acc[NS / 2];
+        uint32_t it = 0;
+        mbar_wait(bar_w, 0);  // resident weights have landed (TMA complete_tx)
+        for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+            for (int kc = 0; kc < nk; ++kc, ++it) {
+                const int s = it % nst;
+                mbar_wait(bar_full(s), (it / nst) & 1);
+                const uint32_t a_hi = smem_u + (uint32_t)s * T2_STAGE_BYTES + (uint32_t)g * (64 * 128);
+                const uint32_t a_lo = a_hi + T2_A_BYTES;
+                const uint32_t b_hi = wres_u32 + (uint32_t)(kc * 2) * (NS * T2_KC * 4);
+                const uint32_t b_lo = b_hi + NS * T2_KC * 4;
+                wg_reg_fence(acc);
+                wg_fence();
 #pragma unroll
-                    for (int itr = 0; itr < 8; ++itr) {
-                        const int rw = itr * 4 + rr;
-                        yv[itr] = rw < nv ? __ldg(reinterpret_cast<const float4*>(
-                                                p.e_y + (row0 + rw) * p.e_ldy + col0 + 4 * c4))
-                                          : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
+                for (int ks = 0; ks < T2_KC / 8; ++ks) {
+                    const uint32_t ko = ks * 32;
+                    const uint64_t dah = wg_desc_k_sw128(a_hi + ko), dal = wg_desc_k_sw128(a_lo + ko);
+                    const uint64_t dbh = wg_desc_k_sw128(b_hi + ko), dbl = wg_desc_k_sw128(b_lo + ko);
+                    wgmma_tf32<NS>(acc, dah, dbh, (kc | ks) ? 1u : 0u);
+                    wgmma_tf32<NS>(acc, dal, dbh, 1u);
+                    wgmma_tf32<NS>(acc, dah, dbl, 1u);
                 }
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(w * 32) << 16) + (uint32_t)(a * NS + cb * 32), r);
-                // lane = row -> shared tile -> (4 rows x 128 B) per store instruction
-#pragma unroll
-                for (int j = 0; j < 8; ++j)
-                    *reinterpret_cast<float4*>(tile_s + lane * T2_EPI_PITCH + 4 * j) =
-                        make_float4(__uint_as_float(r[4 * j]) + bias_s[cb * 32 + 4 * j],
-                                    __uint_as_float(r[4 * j + 1]) + bias_s[cb * 32 + 4 * j + 1],
-                                    __uint_as_float(r[4 * j + 2]) + bias_s[cb * 32 + 4 * j + 2],
-                                    __uint_as_float(r[4 * j + 3]) + bias_s[cb * 32 + 4 * j + 3]);
+                wg_commit();
+                wg_wait<0>();
+                wg_reg_fence(acc);
                 __syncwarp();
-                float4 e_sc, e_sh, e_mu, e_rs;
-                float b1[4] = {0.f, 0.f, 0.f, 0.f}, b2[4] = {0.f, 0.f, 0.f, 0.f};
-                if (p.epi == EPI_BNRED) {
-                    e_sc = *reinterpret_cast<const float4*>(ev_s + cb * 32 + 4 * c4);
-                    e_sh = *reinterpret_cast<const float4*>(ev_s + NS + cb * 32 + 4 * c4);
-                    e_mu = *reinterpret_cast<const float4*>(ev_s + 2 * NS + cb * 32 + 4 * c4);
-                    e_rs = *reinterpret_cast<const float4*>(ev_s + 3 * NS + cb * 32 + 4 * c4);
-                }
+                if (lane == 0) mbar_arrive(bar_empty(s));
+            }
+            // ---- epilogue: this thread holds rows ra = row0 + r and rb = ra + 8, column pairs 8j + cq
+            const int64_t row0 = tile * T2_BM + g * 64 + wl * 16;
+            const int nv = (int)max((int64_t)0, min((int64_t)16, p.M - row0));
+            const bool va = r < nv, vb = r + 8 < nv;
+            float* ca = p.C + (row0 + r) * p.ldc + n0;
+            float* cb = ca + 8 * p.ldc;
 #pragma unroll
-                for (int itr = 0; itr < 8; ++itr) {
-                    const int rw = itr * 4 + rr;
-                    const float4 o = *reinterpret_cast<const float4*>(tile_s + rw * T2_EPI_PITCH + 4 * c4);
-                    if (rw < nv) {
-                        *reinterpret_cast<float4*>(p.C + (row0 + rw) * p.ldc + col0 + 4 * c4) = o;
-                        if (p.epi == EPI_BNRED) {
-                            // BatchNorm-backward sums of the layer below: gz = relu'(y) * g
-                            const float4 y = yv[itr];
-                            float gx = o.x, gy = o.y, gz = o.z, gw = o.w;
-                            if (p.e_relu) {
-                                if (!(fmaf(y.x, e_sc.x, e_sh.x) > 0.f)) gx = 0.f;
-                                if (!(fmaf(y.y, e_sc.y, e_sh.y) > 0.f)) gy = 0.f;
-                                if (!(fmaf(y.z, e_sc.z, e_sh.z) > 0.f)) gz = 0.f;
-                                if (!(fmaf(y.w, e_sc.w, e_sh.w) > 0.f)) gw = 0.f;
-                            }
-                            b1[0] += gx; b1[1] += gy; b1[2] += gz; b1[3] += gw;
-                            b2[0] = fmaf(gx, (y.x - e_mu.x) * e_rs.x, b2[0]);
-                            b2[1] = fmaf(gy, (y.y - e_mu.y) * e_rs.y, b2[1]);
-                            b2[2] = fmaf(gz, (y.z - e_mu.z) * e_rs.z, b2[2]);
-                            b2[3] = fmaf(gw, (y.w - e_mu.w) * e_rs.w, b2[3]);
+            for (int j = 0; j < NS / 8; ++j) {
+                const int c = 8 * j + cq;
+                const float2 oa = make_float2(acc[4 * j] + bias_s[c], acc[4 * j + 1] + bias_s[c + 1]);
+                const float2 ob = make_float2(acc[4 * j + 2] + bias_s[c], acc[4 * j + 3] + bias_s[c + 1]);
+                if (va) *reinterpret_cast<float2*>(ca + c) = oa;
+                if (vb) *reinterpret_cast<float2*>(cb + c) = ob;
+                if (p.epi == EPI_BNRED) {
+                    // BatchNorm-backward sums of the layer below: gz = relu'(y) * g
+                    const float2 ya = va ? __ldg(reinterpret_cast<const float2*>(p.e_y + (row0 + r) * p.e_ldy + n0 + c))
+                                         : make_float2(0.f, 0.f);
+                    const float2 yb = vb ? __ldg(reinterpret_cast<const float2*>(p.e_y + (row0 + r + 8) * p.e_ldy + n0 + c))
+                                         : make_float2(0.f, 0.f);
+                    float b1[2], b2[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float esc = ev_s[c + e], esh = ev_s[NS + c + e];
+                        const float emu = ev_s[2 * NS + c + e], ers = ev_s[3 * NS + c + e];
+                        const float y0 = e ? ya.y : ya.x, y1 = e ? yb.y : yb.x;
+                        float g0 = va ? (e ? oa.y : oa.x) : 0.f, g1 = vb ? (e ? ob.y : ob.x) : 0.f;
+                        if (p.e_relu) {
+                            if (!(fmaf(y0, esc, esh) > 0.f)) g0 = 0.f;
+                            if (!(fmaf(y1, esc, esh) > 0.f)) g1 = 0.f;
                         }
+                        b1[e] = g0 + g1;
+                        b2[e] = fmaf(g1, (y1 - emu) * ers, g0 * ((y0 - emu) * ers));
                     }
-                }
-                if (p.epi == EPI_BNRED) {
-                    // lanes (rr, c4) with the same c4 hold the same 4 columns: fold the 4 row groups
+                    // lanes with the same lane % 4 hold the same columns: fold the 8 row pairs
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        b1[k] += __shfl_xor_sync(0xffffffffu, b1[k], 8);
-                        b1[k] += __shfl_xor_sync(0xffffffffu, b1[k], 16);
-                        b2[k] += __shfl_xor_sync(0xffffffffu, b2[k], 8);
-                        b2[k] += __shfl_xor_sync(0xffffffffu, b2[k], 16);
-                    }
-                    if (rr == 0) {
+                    for (int e = 0; e < 2; ++e)
 #pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            float* o = acc_w + (cb * 32 + 4 * c4 + k) * 4;
-                            o[0] += b1[k];
-                            o[1] += b2[k];
+                        for (int o = 4; o < 32; o <<= 1) {
+                            b1[e] += __shfl_xor_sync(0xffffffffu, b1[e], o);
+                            b2[e] += __shfl_xor_sync(0xffffffffu, b2[e], o);
+                        }
+                    if (r == 0) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float* o = acc_w + (c + e) * 4;
+                            o[0] += b1[e];
+                            o[1] += b2[e];
                         }
                     }
                 }
                 if (p.epi == EPI_STATS && nv > 0) {
-                    // per-column pivoted sums over the valid rows of this warp's 32-row group, read
-                    // back from the transpose tile (lane = column: conflict-free); the pivot is the
-                    // first value the warp ever saw in this column (kept across tiles)
-                    const float* tile_c = tile_s + lane;
-                    float* o = acc_w + (cb * 32 + lane) * 4;
-                    float n_old = o[0], d1 = o[1], d2 = o[2];
-                    const float pivot = n_old > 0.f ? o[3] : tile_c[0];
+                    // per-column pivoted sums over the valid rows of this warp's 16-row group; the pivot
+                    // is the first value the warp ever saw in this column (kept across tiles)
 #pragma unroll
-                    for (int rw = 0; rw < 32; ++rw) {
-                        const float d = tile_c[rw * T2_EPI_PITCH] - pivot;
-                        if (rw < nv) {
-                            d1 += d;
-                            d2 = fmaf(d, d, d2);
+                    for (int e = 0; e < 2; ++e) {
+                        float* o = acc_w + (c + e) * 4;
+                        const float n_old = o[0];
+                        const float first = __shfl_sync(0xffffffffu, e ? oa.y : oa.x, lane & 3);
+                        const float pivot = n_old > 0.f ? o[3] : first;
+                        const float d0 = va ? (e ? oa.y : oa.x) - pivot : 0.f;
+                        const float d1 = vb ? (e ? ob.y : ob.x) - pivot : 0.f;
+                        float s1 = d0 + d1, s2 = fmaf(d1, d1, d0 * d0);
+#pragma unroll
+                        for (int sh = 4; sh < 32; sh <<= 1) {
+                            s1 += __shfl_xor_sync(0xffffffffu, s1, sh);
+                            s2 += __shfl_xor_sync(0xffffffffu, s2, sh);
                         }
+                        __syncwarp();
+                        if (r == 0) {
+                            o[0] = n_old + (float)nv;
+                            o[1] += s1;
+                            o[2] += s2;
+                            o[3] = pivot;
+                        }
+                        __syncwarp();
                     }
-                    o[0] = n_old + (float)nv;
-                    o[1] = d1;
-                    o[2] = d2;
-                    o[3] = pivot;
                 }
-                __syncwarp();
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_accempty(a));
         }
     }
 
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                     "r"((uint32_t)(2 * NS < 32 ? 32 : 2 * NS))
-                     : "memory");
-    }
     if (p.epi == EPI_NONE) return;
 
-    // ---------------- column reductions: CTA partial, then the last CTA merges and folds -------------
+    // ---------------- column reductions: CTA partial, then the merge kernel folds -------------
     if (t < NS) {
         if (p.epi == EPI_STATS) {
-            // Chan merge of the 4 row quarters (each: n, pivot + d1/n, d2 - d1^2/n), fixed order
+            // Chan merge of the 8 row groups (each: n, pivot + d1/n, d2 - d1^2/n), fixed order
             double n = 0.0, mean = 0.0, m2 = 0.0;
 #pragma unroll
             for (int wq = 0; wq < T2_EPI_WARPS; ++wq) {
@@ -540,11 +455,10 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     }
 }
 
-// Second (tiny) kernel of a fused reduction: one warp per column folds the <= 148 per-CTA partials in
+// Second (tiny) kernel of a fused reduction: one warp per column folds the <= kNumSMs per-CTA partials in
 // a fixed order (deterministic) and writes mean/var (+ BatchNorm fold, running statistics) or s1|s2.
-// (An in-kernel grid barrier was tried first: it needs a cooperative launch, which must wait until the
-// WHOLE grid fits on the GPU and thereby serialises against the weight-gradient kernels of the side
-// stream — 2.30 ms per step instead of 1.97.)
+// (An in-kernel grid barrier would need a cooperative launch, which must wait until the WHOLE grid fits
+// on the GPU and thereby serialises against the weight-gradient kernels of the side stream.)
 __global__ void __launch_bounds__(256) tc_merge_kernel(const Tc2Args p, int P) {
     SPG_PDL_ENTRY();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -553,7 +467,7 @@ __global__ void __launch_bounds__(256) tc_merge_kernel(const Tc2Args p, int P) {
     {
         if (p.epi == EPI_STATS) {
             double sn = 0.0, snm = 0.0;
-            float pn[5], pm[5], pq[5];  // P <= 148 -> <= 5 partials per lane
+            float pn[5], pm[5], pq[5];  // P <= kNumSMs <= 160 -> <= 5 partials per lane
 #pragma unroll
             for (int u = 0; u < 5; ++u) {
                 const int k = lane + 32 * u;
@@ -650,8 +564,7 @@ static int make_weight_map(CUtensorMap* map, const float* image, int N, int K, i
 }
 
 static inline int fixed_smem(int NS, int K) {
-    return (K / T2_KC) * 2 * NS * T2_KC * 4 + (4 * K + NS + 4 * NS + T2_EPI_WARPS * NS * 4) * 4 +
-           T2_EPI_WARPS * 32 * T2_EPI_PITCH * 4;
+    return (K / T2_KC) * 2 * NS * T2_KC * 4 + (4 * K + NS + 4 * NS + T2_EPI_WARPS * NS * 4) * 4;
 }
 
 static inline int stages_for(int NS, int K) {

@@ -1,4 +1,4 @@
-// Weight images of the tcgen05 GEMMs (tc_gemm2.cu): pre-split (tf32 hi / lo) and pre-swizzled copies
+// Weight images of the wgmma GEMMs (tc_gemm2.cu): pre-split (tf32 hi / lo) and pre-swizzled copies
 // of a weight matrix in exactly the shared-memory layout the MMA reads, so that the resident-weight
 // load of the GEMM is a plain TMA box copy.
 //

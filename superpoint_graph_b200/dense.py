@@ -176,7 +176,7 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
     `grads` (list aligned with params) is filled in place.  Returns the gradient w.r.t. the
     chain input's activated value [M, cin_0] (or None).
 
-    Where the data-gradient GEMM of a layer runs on the tcgen05 kernel, the BatchNorm/ReLU backward
+    Where the data-gradient GEMM of a layer runs on the wgmma kernel, the BatchNorm/ReLU backward
     around it is fused into that ONE launch: the prologue turns dL/d(activation) into dL/dY on the
     fly (and stores it once for the weight-gradient kernel), the epilogue reduces the BatchNorm-
     backward sums of the layer below from the tile it has just produced.  The stand-alone

@@ -1,4 +1,4 @@
-"""Installs the sm_100a operators under the reference's module names.
+"""Installs the sm_90a operators under the reference's module names.
 
 The reference's trainer does `from learning import spg, graphnet, pointnet, metrics` and
 `import ecc`-style imports (ref: learning/main.py:31-37, learning/spg.py:21, learning/modules.py:14,

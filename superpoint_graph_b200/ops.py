@@ -19,7 +19,7 @@ def _need_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "superpoint_graph_b200 ops run on sm_100a CUDA tensors only (got a CPU tensor); "
+                "superpoint_graph_b200 ops run on sm_90a CUDA tensors only (got a CPU tensor); "
                 "there is no CPU fallback")
 
 
@@ -299,9 +299,9 @@ GEMM_FLOPS = [0]  # algorithmic FLOPs (2*M*N*K) issued through gemm(); read by b
 
 def _auto_split(M, N, K):
     tiles = ((M + 127) // 128) * ((N + 63) // 64)
-    if tiles >= 148 or K < 256:
+    if tiles >= 132 or K < 256:
         return 1
-    split = min((2 * 148 + tiles - 1) // tiles, max(1, K // 64))
+    split = min((2 * 132 + tiles - 1) // tiles, max(1, K // 64))
     return max(1, split)
 
 
@@ -354,7 +354,7 @@ def gemm(A, lda, a_kmajor, B, ldb, b_kmajor, M, N, K, bias=None, out=None, ldc=N
     return out
 
 
-USE_TC = [os.environ.get("SPG_TC", "1") != "0"]  # tcgen05 path for the large point-wise layers
+USE_TC = [os.environ.get("SPG_TC", "1") != "0"]  # tensor-core (wgmma) path for the large point-wise layers
 USE_FUSED_RNN = [os.environ.get("SPG_FUSED_RNN", "1") != "0"]  # one-kernel R x {ECC, cell} loop
 USE_FUSED_BNBWD = [os.environ.get("SPG_FUSED_BNBWD", "1") != "0"]  # BatchNorm backward inside the dX GEMM (prologue + epilogue sums)
 USE_FUSED_EVAL = [os.environ.get("SPG_FUSED_EVAL", "1") != "0"]  # eval-mode PointNet trunk as one kernel per chain
@@ -418,7 +418,7 @@ def _weight_image(W, ldw, transpose, N, K, kv, dev):
 
 def tc_gemm(A, lda, W, ldw, transpose, M, N, K, bias=None, a_aff=None, stats=False, k_valid=None,
             fold=None, bnbwd=None, bnred=None):
-    """C[M,N] = f(A)[M,K] B[N,K]^T + bias on the tcgen05 3xTF32 kernel (spg_tc_gemm_ex).
+    """C[M,N] = f(A)[M,K] B[N,K]^T + bias on the wgmma 3xTF32 kernel (spg_tc_gemm_ex).
     transpose=False: B = W ([N,K], ld ldw); True: B = W^T with W [K,N].
 
     stats / fold: batch statistics of C (and the BatchNorm fold) finished inside the kernel; returns
@@ -479,7 +479,7 @@ def tc_gemm(A, lda, W, ldw, transpose, M, N, K, bias=None, a_aff=None, stats=Fal
     return res[0] if len(res) == 1 else tuple(res)
 
 
-MAX_TC_PARTIALS = [148]  # spg_tc_gemm_max_partials(): CTAs along the rows = partials per column
+MAX_TC_PARTIALS = [132]  # spg_tc_gemm_max_partials(): CTAs along the rows = partials per column
 
 TC_FLOPS = [0]  # algorithmic FLOPs through tc_gemm (forward + data gradients)
 DW_FLOPS = [0]  # algorithmic FLOPs through tc_dw (weight gradients)
@@ -491,7 +491,7 @@ def tc_dw_supported(M, co, ci, lddy, ldp):
 
 
 def tc_dw(dY, lddy, P, ldp, M, co, ci, p_aff=None):
-    """dW[co,ci] = dY^T [co,M] f(P)[M,ci] on the tcgen05 3xTF32 kernel (ci may be the padded
+    """dW[co,ci] = dY^T [co,M] f(P)[M,ci] on the wgmma 3xTF32 kernel (ci may be the padded
     leading dimension of P; the caller slices the valid columns)."""
     _need_cuda(dY, P)
     dev = dY.device

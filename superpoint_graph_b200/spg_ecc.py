@@ -1,4 +1,4 @@
-"""Edge-conditioned convolution with the reference's `learning/ecc` API on the sm_100a kernels.
+"""Edge-conditioned convolution with the reference's `learning/ecc` API on the sm_90a kernels.
 
 Mirrors (names, argument order, defaults, error behaviour):
   GraphConvInfo      ref: learning/ecc/GraphConvInfo.py:16-86

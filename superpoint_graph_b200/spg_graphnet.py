@@ -3,7 +3,7 @@
 The `model_config` mini-language is parsed with the reference's semantics — including the trap
 that the third `gru_` token is `vv` (graphnet.py:68) although main.py's help text calls it `mv` —
 and modules are registered under the same names (`'0'`, `'1'`, ...) so state dicts interchange.
-Consecutive `f`/`b`/`r`/`d` tokens run as one fused Linear/BN/ReLU chain on the sm_100a kernels.
+Consecutive `f`/`b`/`r`/`d` tokens run as one fused Linear/BN/ReLU chain on the sm_90a kernels.
 """
 import torch.nn as nn
 import torch.nn.init as init

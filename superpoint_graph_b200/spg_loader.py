@@ -5,7 +5,7 @@ Reference: learning/spg.py:130-170 (`loader`: one `load_superpoint` per graph no
 selection), :238-260 (`augment_cloud`).  There every superpoint is one HDF5 dataset read, a handful
 of numpy calls and a host->device copy of the finished [Nv, F, L] tensor (7 KB per superpoint per
 step).  Here the parsed points live in HBM once (`SuperpointStore`: one packed [rows, C] array —
-all of S3DIS is a few GB, 180 GB are available), the host only decides WHICH rows (ids, sample
+all of S3DIS is a few GB, an H100 has 80 GB), the host only decides WHICH rows (ids, sample
 indices: 0.5 KB per superpoint) and one kernel (`spg_cloud_build`, csrc/loader.cu) emits the
 tensor PointNet reads.  With the host-drawn indices the output is bit-identical to the
 reference's; `device_rng=True` moves the draws onto the GPU as well (same distribution, not the

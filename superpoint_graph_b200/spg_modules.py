@@ -1,5 +1,5 @@
 """Recurrent ECC module and GRUCellEx with the reference's signatures (ref:
-learning/modules.py:128-183, 205-259), executed as ONE autograd node over the sm_100a kernels:
+learning/modules.py:128-183, 205-259), executed as ONE autograd node over the sm_90a kernels:
 
   filters  = fnet(edge features)                      (once, fused Linear/BN/ReLU chain)
   repeat R: input = ECC(h, filters); h = GRUCellEx(input, h)
@@ -141,7 +141,7 @@ class RNNGraphConvModule(nn.Module):
         self.use_pyg = use_pyg
         if use_pyg:
             raise NotImplementedError(
-                "use_pyg=1 selects the reference's torch_geometric path; the sm_100a kernels "
+                "use_pyg=1 selects the reference's torch_geometric path; the sm_90a kernels "
                 "implement the native ECC path (use --use_pyg 0)")
         if self._isLSTM:
             raise NotImplementedError("lstm_* model configs are outside the accelerated path")

@@ -1,5 +1,5 @@
 """PointNet / STNkD / CloudEmbedder with the reference's operator signatures on top of the
-sm_100a kernels.
+sm_90a kernels.
 
 Drop-in for `learning/pointnet.py` (ref: learning/pointnet.py:16-218): same class names,
 constructor arguments, attribute names (`stn`, `convs`, `fcs`, `proj`, `nfeat_stn`), parameter
@@ -481,9 +481,8 @@ class CloudEmbedder():
         clouds, clouds_global, idx_valid = self._prep(clouds_flag, clouds, clouds_global)
         return self._embed_monger(model, clouds, clouds_global, idx_valid, clouds_flag.size(0))
 
-    # measured (tools/pipe_probe.py, B200 + PCIe host link): 115 MB / 20 000 superpoints 6.3 ms as one copy,
-    # 4.85 ms in 4 chunks; 42 MB / 8192 superpoints 2.6 -> 1.9 ms in 3; more chunks make the step issue-bound
-    # on the host (every chunk is ~25 launches)
+    # Large uploads go in a few chunks so that the forward of chunk i overlaps the copy of chunk i+1; more
+    # chunks make the step issue-bound on the host (every chunk is ~25 launches)
     PIPELINE_MIN_BYTES = 16 << 20
     PIPELINE_CHUNK_BYTES = 14 << 20
     PIPELINE_CHUNKS = 4

@@ -1,4 +1,4 @@
-"""The training / inference step of the reference's trainer on the sm_100a path.
+"""The training / inference step of the reference's trainer on the sm_90a path.
 
 What `learning/main.py:189-221` does per batch — set_info, zero_grad, PointNet embedding, graph
 network, weighted cross entropy, backward, element-wise gradient clamp, Adam, logits to the host —
@@ -168,9 +168,8 @@ class Trainer(object):
     def compute_gradients(self, db):
         """Forward, loss, backward; gathers every parameter gradient into the flat buffer.
         Returns (loss[1], logits).  Purely local to this rank (no collective)."""
-        # launch policy (ops.set_pdl): programmatic dependent launch measured 2 % SLOWER on the training step —
-        # for the whole step and for the forward phase alone (profiles/r2_pdl_policy_ab.log) — so it is off
-        # here; the inference paths leave it on
+        # launch policy (ops.set_pdl): programmatic dependent launch is off on the training step and on for the
+        # inference paths
         ops.set_pdl(0)
         try:
             return self._compute_gradients(db)

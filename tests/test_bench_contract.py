@@ -1,5 +1,5 @@
-"""CPU: the reference arm of bench.py (the reference's own modules from baseline/_ref on the host cores) prints one JSON line with the
-contract's keys; the b200 arm refuses to run without a CUDA device (no CPU fallback)."""
+"""CPU: the reference arm of bench.py (the oracle's port of the reference's CPU path on the host cores) prints one JSON line
+with the contract's keys; the b200 arm refuses to run without a CUDA device (no CPU fallback)."""
 import json
 import os
 import subprocess
@@ -18,8 +18,7 @@ def test_reference_arm_json_line():
     for key in ("impl", "metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step",
                 "higher_is_better", "scaling", "vs_baseline", "dtype", "data", "config", "cpu_baseline", "e2e"):
         assert key in line, key
-    have_ref = os.path.exists(os.path.join(ROOT, "baseline", "_ref", "learning", "pointnet.py"))
-    assert line["impl"] == "reference" and line["cpu_baseline"]["kind"] == ("reference" if have_ref else "port")
+    assert line["impl"] == "reference" and line["cpu_baseline"]["kind"] == "port"
     assert line["cpu_baseline"]["nproc"] >= line["cpu_baseline"]["cores"] >= 1
     assert set(line["config"]) == {"workload", "parallelism", "l2", "superpoints", "embedded_superpoints",
                                    "points", "edges"}

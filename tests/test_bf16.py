@@ -1,4 +1,4 @@
-"""bf16 arithmetic of the PointNet trunk (BASELINE configs[3]: "bf16"): tcgen05 kind::f16, bf16 operands,
+"""bf16 arithmetic of the PointNet trunk (BASELINE configs[3]: "bf16"): wgmma on bf16 operands,
 fp32 accumulation, activations rounded to bf16 between layers.  Checked against the fp32 oracle with a
 STATED tolerance: five layers of bf16 rounding (2^-9 relative per operand) give ~1e-2 of the output scale;
 the bound is 3e-2 on the PointNet outputs and on the logits of a whole inference step.  The fp32 (3xTF32)

@@ -3,7 +3,7 @@ the configurations bench.py times — not miniatures of them — against the pin
 same Trainer / CloudEmbedder / C-ABI path the bench uses.
 
 Tolerances: logits and loss 1e-4 relative (north_star).  The oracle runs in float64 here.
-Gradients (measured against that float64 truth: profiles/r2_grad_diag.log, tools/grad_diag.py):
+Gradients (against that float64 truth):
   * everything that is not a point-wise-layer parameter agrees to <= 1e-5 of the tensor's largest
     gradient (bound here: 3e-3; 1e-2 below the filter network's BatchNorm at 1e5 edges);
   * the point-wise layers sit UNDER a max-pool over 128 points: a cloud/channel pair whose two largest
