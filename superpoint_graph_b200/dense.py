@@ -26,10 +26,13 @@ class LayerSpec(object):
         self.bn, self.relu, self.cin, self.cout = bn, relu, cin, cout
 
 
-def parse_sequential(seq, training):
+def parse_sequential(seq, training, params=None):
     """nn.Sequential -> ([LayerSpec], [parameter tensors]).  LayerSpec.w/b/gamma/beta are
-    positions in the returned parameter list; LayerSpec.bn is the BatchNorm module (buffers)."""
-    specs, params = [], []
+    positions in the returned parameter list; LayerSpec.bn is the BatchNorm module (buffers).
+    With `params` given, the parameters are appended to that list (and it is returned), so that
+    several chains index one flat list."""
+    specs = []
+    params = [] if params is None else params
     mods = list(seq.children()) if isinstance(seq, nn.Sequential) else list(seq)
     i = 0
     while i < len(mods):

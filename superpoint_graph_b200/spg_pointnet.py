@@ -12,21 +12,32 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .dense import Deferred, chain_backward, chain_forward, parse_sequential
+from .dense import Deferred, _w2d, chain_backward, chain_forward, parse_sequential
 
 
-def _conv_stack(nfeat, widths, norm, n_group):
+def _norm_relu(norm, w, n_group):
+    """The normalisation the reference's `norm` argument selects for a layer of width w, then its ReLU."""
     mods = []
-    for i, w in enumerate(widths):
-        mods.append(nn.Conv1d(widths[i - 1] if i > 0 else nfeat, w, 1))
-        if norm == 'batch':
-            mods.append(nn.BatchNorm1d(w))
-        elif norm == 'layer':
-            mods.append(nn.GroupNorm(1, w))
-        elif norm == 'group':
-            mods.append(nn.GroupNorm(n_group, w))
-        mods.append(nn.ReLU(True))
+    if norm == 'batch':
+        mods.append(nn.BatchNorm1d(w))
+    elif norm == 'layer':
+        mods.append(nn.GroupNorm(1, w))
+    elif norm == 'group':
+        mods.append(nn.GroupNorm(n_group, w))
+    return mods + [nn.ReLU(True)]
+
+
+def _stack(layer, nin, widths, norm, n_group):
+    """nn.Sequential of layer(nin, widths[0]), norm, ReLU, layer(widths[0], widths[1]), norm, ReLU, ..."""
+    mods = []
+    for w in widths:
+        mods += [layer(nin, w)] + _norm_relu(norm, w, n_group)
+        nin = w
     return nn.Sequential(*mods)
+
+
+def _conv1x1(nin, nout):
+    return nn.Conv1d(nin, nout, 1)
 
 
 def _round4(n):
@@ -44,18 +55,8 @@ class STNkD(nn.Module):
 
     def __init__(self, nfeat, nf_conv, nf_fc, K=2, norm='batch', affine=True, n_group=1):
         super(STNkD, self).__init__()
-        self.convs = _conv_stack(nfeat, nf_conv, norm, n_group)
-        mods = []
-        for i, w in enumerate(nf_fc):
-            mods.append(nn.Linear(nf_fc[i - 1] if i > 0 else nf_conv[-1], w))
-            if norm == 'batch':
-                mods.append(nn.BatchNorm1d(w))
-            elif norm == 'layer':
-                mods.append(nn.GroupNorm(1, w))
-            elif norm == 'group':
-                mods.append(nn.GroupNorm(n_group, w))
-            mods.append(nn.ReLU(True))
-        self.fcs = nn.Sequential(*mods)
+        self.convs = _stack(_conv1x1, nfeat, nf_conv, norm, n_group)
+        self.fcs = _stack(nn.Linear, nf_conv[-1], nf_fc, norm, n_group)
         self.proj = nn.Linear(nf_fc[-1], K * K)
         nn.init.constant_(self.proj.weight, 0)
         nn.init.constant_(self.proj.bias, 0)
@@ -67,64 +68,165 @@ class STNkD(nn.Module):
         """input [B, nfeat, L] -> [B, K, K] (= proj(...) + I)."""
         if self.eye.device != input.device:
             self.eye = self.eye.to(input.device)
-        T = _StnFunction.apply(input, self, self.training, *_stn_params(self, self.training)[1])
+        params = []
+        groups = _stn_groups(self, self.training, params)
+        T = _StnFunction.apply(input, groups, self.training, *params)
         return T.view(-1, self._K, self._K) + self.eye
 
 
-def _stn_params(stn, training):
-    """(spec groups, flat parameter list) for convs | fcs+proj of an STNkD."""
-    cs, cp = parse_sequential(stn.convs, training)
-    fs, fp = parse_sequential(list(stn.fcs.children()) + [stn.proj], training)
-    off = len(cp)
-    for sp in fs:
-        sp.w += off
-        if sp.b is not None:
-            sp.b += off
-        if sp.gamma is not None:
-            sp.gamma += off
-            sp.beta += off
-    return (cs, fs), cp + fp
+def _stn_groups(stn, training, params):
+    """Spec groups (convs, fcs+proj) of an STNkD; its parameters are appended to `params`."""
+    cs, _ = parse_sequential(stn.convs, training, params)
+    fs, _ = parse_sequential(list(stn.fcs.children()) + [stn.proj], training, params)
+    return cs, fs
 
 
-def _stn_forward(rows, ld, B, L, groups, params, training, saved):
-    """rows: raw point rows [B*L, ld]; returns flat T [B, K*K] (without the identity)."""
+# Segment layouts: everything of the PointNet forward/backward that depends on how the points of a
+# cloud are laid out.  Point rows are [M, ld] (one point per row, features zero-padded to ld).
+class _Clouds(object):
+    """Fixed-length clouds [B, F, L] (the reference's layout); point row b*L + l is point l of cloud b."""
+
+    has_input_grad = True
+
+    def __init__(self, clouds):
+        self.clouds = clouds.contiguous()
+        self.device = clouds.device
+        self.B, self.F, self.L = self.clouds.shape
+        self.M = self.B * self.L
+        self.ld = _row_ld(self.F)
+
+    def rows(self, T=None):
+        """The point rows; with T [B, 4] the xy columns are transformed by T + I."""
+        return ops.cloud_rows(self.clouds, T, self.ld, add_eye=T is not None)
+
+    def segmax(self, out, pooled):
+        """Max over each cloud's points of the Deferred point rows `out` into pooled[:, :out.C]; returns argmax."""
+        return ops.segmax_fwd(out.raw, out.ld, self.B, self.L, out.C, out.scale, out.shift, out.relu, pooled,
+                              pooled.shape[1])
+
+    def segmax_backward(self, g_pool, specs, params, record, need_input_grad, grads):
+        """Backward of segmax and of the point-wise chain `specs` before it; returns the point-row gradient."""
+        saved, argmax = record
+        # chain_backward fuses the pool backward into the last layer's BatchNorm backward
+        return chain_backward(None, specs[-1].cout, self.M, specs, params, saved, need_input_grad, grads,
+                              pooled=(g_pool, g_pool.shape[1], argmax, self.B, self.L))
+
+    def xy_transform_backward(self, g_rows):
+        """dT [B, 4] from the gradient w.r.t. the transformed point rows."""
+        return ops.stn_apply_bwd(self.clouds, g_rows, g_rows.shape[1])
+
+    def input_grad(self, g_rows):
+        """The point-row gradient as [B, F, L]."""
+        return ops.rows_to_clouds(g_rows, g_rows.shape[1], self.B, self.F, self.L)
+
+    def fused_eval_ok(self, groups, params, nfeat_stn):
+        """Whether an eval-mode forward can run each point-wise chain as one fused trunk kernel."""
+        stn_g, conv_g, _ = groups
+        if not conv_g or (nfeat_stn > 0 and nfeat_stn != self.F):
+            return False
+        chains = [conv_g] + ([stn_g[0]] if nfeat_stn > 0 else [])
+        return all(_conv_layers(specs, params) is not None
+                   and ops.pointnet_fused_supported(self.F, self.L, [sp.cout for sp in specs]) for specs in chains)
+
+    def fused_pool(self, specs, params, T, pooled):
+        """Eval-mode segmax of the chain `specs` over the (T-transformed) clouds in one kernel
+        (csrc/pointnet_fused.cu: input tile to pooled row on chip, activations never in HBM)."""
+        img, bias, widths = ops.pointnet_fused_image(_conv_layers(specs, params), self.F, bf16=ops.EVAL_BF16[0])
+        ops.pointnet_fused_eval(self.clouds, T, img, bias, widths, pooled, pooled.shape[1])
+
+
+class _Segments(object):
+    """Ragged superpoints as CSR segments: `points` [P, F] of all B superpoints back to back, int64
+    `offsets` [B+1]; point row p is points[p]."""
+
+    has_input_grad = False  # the points are data: no caller asks for their gradient
+
+    def __init__(self, points, offsets):
+        self.offsets = offsets.to(torch.int64).contiguous()
+        self.device = points.device
+        self.M, self.F = points.shape
+        self.B = self.offsets.numel() - 1
+        self.ld = _row_ld(self.F)
+        self.rows0 = torch.empty((self.M, self.ld), dtype=torch.float32, device=self.device)
+        ops.zero_(self.rows0)
+        ops.affine_act(points.contiguous(), self.F, self.M, self.F, out=self.rows0, ldo=self.ld)
+        # segment of every point row; built before any chain is queued, as it waits for the device
+        self.row_seg = torch.repeat_interleave(torch.arange(self.B, device=self.device, dtype=torch.int32),
+                                               self.offsets[1:] - self.offsets[:-1])
+
+    def rows(self, T=None):
+        if T is None:
+            return self.rows0
+        return ops.rows_xy_transform(self.rows0, T, self.row_seg, add_eye=True)
+
+    def segmax(self, out, pooled):
+        return ops.segmax_csr_fwd(out.raw, out.ld, self.offsets, out.C, out.scale, out.shift, out.relu, pooled,
+                                  pooled.shape[1])
+
+    def segmax_backward(self, g_pool, specs, params, record, need_input_grad, grads):
+        saved, argmax = record
+        C = specs[-1].cout
+        G = ops.segmax_csr_bwd(g_pool, g_pool.shape[1], argmax, self.M, C)
+        return chain_backward(G, C, self.M, specs, params, saved, need_input_grad, grads, own_g=True)
+
+    def xy_transform_backward(self, g_rows):
+        return ops.rows_xy_transform_bwd(self.rows0, g_rows, self.offsets)
+
+    def fused_eval_ok(self, groups, params, nfeat_stn):
+        return False  # the fused trunk kernel reads fixed-length clouds
+
+
+def _conv_layers(specs, params):
+    """[(W2d, bias, bn)] of a parsed Conv1d(k=1)+BatchNorm+ReLU chain, or None if it is not of that form."""
+    out = []
+    for sp in specs:
+        if sp.bn is None or not sp.relu or not sp.bn.track_running_stats or sp.bn.running_mean is None:
+            return None
+        out.append((_w2d(params[sp.w]), params[sp.b] if sp.b is not None else None, sp.bn))
+    return out
+
+
+def _pool(layout, T, specs, params, training, fused, pooled):
+    """Point-wise chain `specs` over the layout's point rows (xy-transformed by T + I if T is given),
+    max-pooled per cloud into pooled[:, :C].  Returns what its backward needs, (layer records, argmax),
+    in training mode."""
+    if fused:
+        layout.fused_pool(specs, params, T, pooled)
+        return None
+    sv = [] if training else None
+    out = chain_forward(Deferred(layout.rows(T), layout.ld, specs[0].cin), layout.M, specs, params, training, sv)
+    argmax = layout.segmax(out, pooled)
+    return (sv, argmax) if training else None
+
+
+def _stn_forward(layout, groups, params, training, fused, saved):
+    """STN conv chain, max-pool, FC chain + proj; returns flat T [B, K*K] (without the identity)."""
     cs, fs = groups
-    M = B * L
-    nfeat = cs[0].cin
-    sv_c = [] if saved is not None else None
-    out = chain_forward(Deferred(rows, ld, nfeat), M, cs, params, training, sv_c)
-    Cs = out.C
-    pooled = torch.empty((B, Cs), dtype=torch.float32, device=rows.device)
-    argmax = ops.segmax_fwd(out.raw, out.ld, B, L, Cs, out.scale, out.shift, out.relu, pooled, Cs)
-    sv_f = [] if saved is not None else None
-    t = chain_forward(Deferred(pooled, Cs, Cs), B, fs, params, training, sv_f)
-    T = t.materialise(B)
-    if saved is not None:
-        saved.update(stn_c=sv_c, stn_f=sv_f, stn_argmax=argmax, stn_Cs=Cs)
+    B, Cs = layout.B, cs[-1].cout
+    pooled = torch.empty((B, Cs), dtype=torch.float32, device=layout.device)
+    conv = _pool(layout, None, cs, params, training, fused, pooled)
+    sv_f = [] if training else None
+    T = chain_forward(Deferred(pooled, Cs, Cs), B, fs, params, training, sv_f).materialise(B)
+    if training:
+        saved.update(stn_c=conv, stn_f=sv_f)
     return T
 
 
-def _stn_backward(dT, B, L, groups, params, saved, grads):
+def _stn_backward(layout, dT, groups, params, saved, grads):
     cs, fs = groups
-    Cs = saved["stn_Cs"]
-    g_pool = chain_backward(dT, dT.shape[1], B, fs, params, saved["stn_f"], True, grads)
-    chain_backward(None, Cs, B * L, cs, params, saved["stn_c"], False, grads,
-                   pooled=(g_pool, Cs, saved["stn_argmax"], B, L))
+    g_pool = chain_backward(dT, dT.shape[1], layout.B, fs, params, saved["stn_f"], True, grads)
+    layout.segmax_backward(g_pool, cs, params, saved["stn_c"], False, grads)
 
 
 class _StnFunction(torch.autograd.Function):
     """Stand-alone STN (used by STNkD.forward and LocalCloudEmbedder)."""
 
     @staticmethod
-    def forward(ctx, clouds, stn, training, *params):
-        clouds = clouds.contiguous()
-        B, F, L = clouds.shape
-        groups, _ = _stn_params(stn, training)
-        ld = _row_ld(F)
-        rows = ops.cloud_rows(clouds, None, ld)
+    def forward(ctx, clouds, groups, training, *params):
+        layout = _Clouds(clouds)
         saved = {} if training else None
-        T = _stn_forward(rows, ld, B, L, groups, params, training, saved)
-        ctx.saved, ctx.groups, ctx.params, ctx.dims = saved, groups, params, (B, L)
+        T = _stn_forward(layout, groups, params, training, False, saved)
+        ctx.saved, ctx.groups, ctx.params, ctx.layout = saved, groups, params, layout
         return T
 
     @staticmethod
@@ -132,9 +234,8 @@ class _StnFunction(torch.autograd.Function):
         if ctx.saved is None:
             raise RuntimeError("backward through an eval-mode forward is not supported")
         grads = [None] * len(ctx.params)
-        B, L = ctx.dims
-        _stn_backward(dT.contiguous(), B, L, ctx.groups, ctx.params, ctx.saved, grads)
-        ctx.saved = None
+        _stn_backward(ctx.layout, dT.contiguous(), ctx.groups, ctx.params, ctx.saved, grads)
+        ctx.saved = ctx.layout = None
         return (None, None, None) + tuple(grads)
 
 
@@ -150,18 +251,12 @@ class PointNet(nn.Module):
         if nfeat_stn > 0:
             self.stn = STNkD(nfeat_stn, nf_conv_stn, nf_fc_stn, norm=norm, n_group=n_group)
         self.nfeat_stn = nfeat_stn
-        self.convs = _conv_stack(nfeat, nf_conv, norm, n_group)
+        self.convs = _stack(_conv1x1, nfeat, nf_conv, norm, n_group)
         mods = []
         for i, w in enumerate(nf_fc):
             mods.append(nn.Linear(nf_fc[i - 1] if i > 0 else nf_conv[-1] + nfeat_global, w))
             if i < len(nf_fc) - 1 or last_ac:
-                if norm == 'batch':
-                    mods.append(nn.BatchNorm1d(w))
-                elif norm == 'layer':
-                    mods.append(nn.GroupNorm(1, w))
-                elif norm == 'group':
-                    mods.append(nn.GroupNorm(n_group, w))
-                mods.append(nn.ReLU(True))
+                mods += _norm_relu(norm, w, n_group)
             if i == len(nf_fc) - 2 and prelast_do > 0:
                 mods.append(nn.Dropout(prelast_do))
         if is_res:
@@ -172,43 +267,32 @@ class PointNet(nn.Module):
         self._nfeat_global = nfeat_global
 
     def _groups(self, training):
-        """Spec groups and the flat parameter list: [stn convs | stn fcs+proj | convs | fcs]."""
+        """Spec groups (stn groups | None, convs, fcs) and the flat parameter list:
+        [stn convs | stn fcs+proj | convs | fcs]."""
         params = []
-        stn_groups = None
-        if self.nfeat_stn > 0:
-            stn_groups, params = _stn_params(self.stn, training)
-            params = list(params)
-        groups = []
-        for seq in (self.convs, self.fcs):
-            sp, pp = parse_sequential(seq, training)
-            off = len(params)
-            for s in sp:
-                s.w += off
-                if s.b is not None:
-                    s.b += off
-                if s.gamma is not None:
-                    s.gamma += off
-                    s.beta += off
-            params += pp
-            groups.append(sp)
-        return stn_groups, groups[0], groups[1], params
+        stn_g = _stn_groups(self.stn, training, params) if self.nfeat_stn > 0 else None
+        conv_g, _ = parse_sequential(self.convs, training, params)
+        fc_g, _ = parse_sequential(self.fcs, training, params)
+        return (stn_g, conv_g, fc_g), params
+
+    def _run(self, x, layout, glob, groups, params):
+        return _PointNetFunction.apply(x, layout, glob, self.nfeat_stn, groups, self.training, *params)
 
     def forward(self, input, input_global):
         """input [B, nfeat, L], input_global [B] | [B, G] | None -> [B, nf_fc[-1]]."""
-        training = self.training
-        stn_g, conv_g, fc_g, params = self._groups(training)
+        groups, params = self._groups(self.training)
+        if input.dtype != torch.float32:
+            raise TypeError("PointNet kernels are float32")
         if input_global is not None:
             input_global = input_global.reshape(input.shape[0], -1).float()
-        if not training and input.shape[0] > _EVAL_CHUNK:
+        if not self.training and input.shape[0] > _EVAL_CHUNK:
             outs = []
             for i in range(0, input.shape[0], _EVAL_CHUNK):
+                x = input[i:i + _EVAL_CHUNK]
                 gl = None if input_global is None else input_global[i:i + _EVAL_CHUNK]
-                outs.append(_PointNetFunction.apply(input[i:i + _EVAL_CHUNK], gl, self.nfeat_stn,
-                                                    (stn_g, conv_g, fc_g), training, *params))
+                outs.append(self._run(x, _Clouds(x), gl, groups, params))
             return torch.cat(outs, 0)
-        return _PointNetFunction.apply(input, input_global, self.nfeat_stn, (stn_g, conv_g, fc_g),
-                                       training, *params)
-
+        return self._run(input, _Clouds(input), input_global, groups, params)
 
     def forward_ragged(self, points, offsets, input_global):
         """Ragged superpoints (north_star; no counterpart in the reference, whose loader resamples every
@@ -217,13 +301,13 @@ class PointNet(nn.Module):
         [B,G] | None.  Same network, same parameters, same BatchNorm semantics (statistics over all P
         points); the max-pool runs over each superpoint's own points.  With equal-length segments the
         result equals `forward` on the [B, nfeat, L] layout."""
-        training = self.training
-        stn_g, conv_g, fc_g, params = self._groups(training)
+        groups, params = self._groups(self.training)
+        if points.dtype != torch.float32 or points.dim() != 2:
+            raise TypeError("ragged PointNet input must be float32 [P, nfeat]")
         B = offsets.numel() - 1
         if input_global is not None:
             input_global = input_global.reshape(B, -1).float()
-        return _PointNetRaggedFunction.apply(points, offsets, input_global, self.nfeat_stn,
-                                             (stn_g, conv_g, fc_g), training, *params)
+        return self._run(points, _Segments(points, offsets), input_global, groups, params)
 
 
 def prepack_weights(ptn, n_clouds, n_points, extra=()):
@@ -234,7 +318,7 @@ def prepack_weights(ptn, n_clouds, n_points, extra=()):
     from .dense import pack_jobs
 
     M = n_clouds * n_points
-    stn_g, conv_g, fc_g, params = ptn._groups(True)
+    (stn_g, conv_g, _), params = ptn._groups(True)
     ld = _row_ld(ptn._nfeat)
     jobs = pack_jobs(conv_g, params, M, ld, ptn.nfeat_stn > 0)
     if stn_g is not None:
@@ -248,47 +332,29 @@ _EVAL_CHUNK = 16384  # clouds per eval-mode slice (bounds the [B*L, 256] activat
 
 
 class _PointNetFunction(torch.autograd.Function):
+    """PointNet forward and backward over a segment layout (_Clouds or _Segments).  `x` is the
+    layout's input tensor; it is an argument so that autograd can route its gradient."""
 
     @staticmethod
-    def forward(ctx, clouds, glob, nfeat_stn, groups, training, *params):
+    def forward(ctx, x, layout, glob, nfeat_stn, groups, training, *params):
         stn_g, conv_g, fc_g = groups
-        clouds = clouds.contiguous()
-        if clouds.dtype != torch.float32:
-            raise TypeError("PointNet kernels are float32")
-        B, F, L = clouds.shape
-        M = B * L
-        ld = _row_ld(F)
-        if not training and _fused_eval_ok(groups, params, F, L, nfeat_stn):
-            ctx.saved = None
-            return _fused_eval_forward(clouds, glob, nfeat_stn, groups, params)
+        B = layout.B
+        fused = not training and layout.fused_eval_ok(groups, params, nfeat_stn)
         saved = {} if training else None
-        T = None
-        if nfeat_stn > 0:
-            rows0 = ops.cloud_rows(clouds, None, ld)
-            T = _stn_forward(rows0, ld, B, L, stn_g, params, training, saved)
-            rows = ops.cloud_rows(clouds, T, ld, add_eye=True)
-            del rows0
-        else:
-            rows = ops.cloud_rows(clouds, None, ld)
-        sv_c = [] if training else None
-        out = chain_forward(Deferred(rows, ld, F), M, conv_g, params, training, sv_c)
-        Ct = out.C
+        T = _stn_forward(layout, stn_g, params, training, fused, saved) if nfeat_stn > 0 else None
+        Ct = conv_g[-1].cout
         G = 0 if glob is None else glob.shape[1]
         ldp = _round4(Ct + G)
-        pooled = torch.empty((B, ldp), dtype=torch.float32, device=clouds.device)
-        argmax = ops.segmax_fwd(out.raw, out.ld, B, L, Ct, out.scale, out.shift, out.relu, pooled,
-                                ldp)
+        pooled = torch.empty((B, ldp), dtype=torch.float32, device=layout.device)
+        conv = _pool(layout, T, conv_g, params, training, fused, pooled)
         if G > 0:
-            glob = glob.contiguous()
-            ops.affine_act(glob, G, B, G, out=pooled[:, Ct:], ldo=ldp)
+            ops.affine_act(glob.contiguous(), G, B, G, out=pooled[:, Ct:], ldo=ldp)
         sv_f = [] if training else None
-        y = chain_forward(Deferred(pooled, ldp, Ct + G), B, fc_g, params, training, sv_f)
-        res = y.materialise(B)
+        res = chain_forward(Deferred(pooled, ldp, Ct + G), B, fc_g, params, training, sv_f).materialise(B)
         if training:
-            saved.update(conv=sv_c, fc=sv_f, argmax=argmax, Ct=Ct, G=G, ld=ld)
-        ctx.saved, ctx.groups, ctx.params = saved, groups, params
-        ctx.dims = (B, F, L, nfeat_stn)
-        ctx.clouds = clouds if (training and nfeat_stn > 0) else None
+            saved.update(conv=conv, fc=sv_f, Ct=Ct, G=G)
+        ctx.saved, ctx.groups, ctx.params, ctx.nfeat_stn = saved, groups, params, nfeat_stn
+        ctx.layout = layout if training else None
         return res
 
     @staticmethod
@@ -297,158 +363,28 @@ class _PointNetFunction(torch.autograd.Function):
             raise RuntimeError("backward through an eval-mode forward is not supported "
                                "(the reference never does it: learning/main.py:229-311)")
         stn_g, conv_g, fc_g = ctx.groups
-        params, saved = ctx.params, ctx.saved
-        B, F, L, nfeat_stn = ctx.dims
+        layout, params, saved, has_stn = ctx.layout, ctx.params, ctx.saved, ctx.nfeat_stn > 0
         grads = [None] * len(params)
         gy = gy.contiguous()
-        Ct, ld = saved["Ct"], saved["ld"]
-        want_clouds, want_glob = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        if want_clouds and nfeat_stn > 0:
+        want_input = ctx.needs_input_grad[0] and layout.has_input_grad
+        if want_input and has_stn:
             raise NotImplementedError("input gradient of a PointNet with an internal STN is not implemented "
                                       "(the reference's callers never ask for it: the clouds are data)")
-        g_pool = chain_backward(gy, gy.shape[1], B, fc_g, params, saved["fc"], True, grads)
+        g_pool = chain_backward(gy, gy.shape[1], layout.B, fc_g, params, saved["fc"], True, grads)
         # gradient w.r.t. the "global" inputs: the tail columns of the pooled row (pointnet.py:128-132)
-        g_glob = g_pool[:, Ct:Ct + saved["G"]].contiguous() if (want_glob and saved["G"] > 0) else None
-        g_rows = chain_backward(None, Ct, B * L, conv_g, params, saved["conv"], nfeat_stn > 0 or want_clouds, grads,
-                                pooled=(g_pool, g_pool.shape[1], saved["argmax"], B, L))
+        Ct, G = saved["Ct"], saved["G"]
+        g_glob = g_pool[:, Ct:Ct + G].contiguous() if (ctx.needs_input_grad[2] and G > 0) else None
+        g_rows = layout.segmax_backward(g_pool, conv_g, params, saved["conv"], has_stn or want_input, grads)
         del g_pool
-        g_clouds = None
-        if nfeat_stn > 0:
-            dT = ops.stn_apply_bwd(ctx.clouds, g_rows, g_rows.shape[1])
+        g_input = None
+        if has_stn:
+            dT = layout.xy_transform_backward(g_rows)
             del g_rows
-            _stn_backward(dT, B, L, stn_g, params, saved, grads)
-        elif want_clouds:  # external transformer (LocalCloudEmbedder): hand the gradient back as [B, F, L]
-            g_clouds = ops.rows_to_clouds(g_rows, g_rows.shape[1], B, F, L)
-        ctx.saved = None
-        ctx.clouds = None
-        return (g_clouds, g_glob, None, None, None) + tuple(grads)
-
-
-def _conv_layers(specs, params):
-    """[(W2d, bias, bn)] of a parsed Conv1d(k=1)+BatchNorm+ReLU chain, or None if it is not of that form."""
-    out = []
-    for sp in specs:
-        if sp.bn is None or not sp.relu or not sp.bn.track_running_stats or sp.bn.running_mean is None:
-            return None
-        W = params[sp.w]
-        W = W.view(W.shape[0], W.shape[1]) if W.dim() == 3 else W
-        out.append((W, params[sp.b] if sp.b is not None else None, sp.bn))
-    return out
-
-
-def _fused_eval_ok(groups, params, F, L, nfeat_stn):
-    stn_g, conv_g, fc_g = groups
-    if not conv_g or _conv_layers(conv_g, params) is None:
-        return False
-    if not ops.pointnet_fused_supported(F, L, [sp.cout for sp in conv_g]):
-        return False
-    if nfeat_stn > 0:
-        if nfeat_stn != F or _conv_layers(stn_g[0], params) is None:
-            return False
-        if not ops.pointnet_fused_supported(F, L, [sp.cout for sp in stn_g[0]]):
-            return False
-    return True
-
-
-def _fused_eval_forward(clouds, glob, nfeat_stn, groups, params):
-    """Eval-mode PointNet with both point-wise chains fused (ops.pointnet_fused_eval: input tile to pooled row
-    on chip); only the [B, C] pooled rows and the small FC chains touch HBM.  ref: pointnet.py:120-133."""
-    stn_g, conv_g, fc_g = groups
-    B, F, L = clouds.shape
-    dev = clouds.device
-    T = None
-    if nfeat_stn > 0:
-        cs, fs = stn_g
-        img, bias, widths = ops.pointnet_fused_image(_conv_layers(cs, params), F, bf16=ops.EVAL_BF16[0])
-        Cs = cs[-1].cout
-        pooled_s = torch.empty((B, Cs), dtype=torch.float32, device=dev)
-        ops.pointnet_fused_eval(clouds, None, img, bias, widths, pooled_s, Cs)
-        T = chain_forward(Deferred(pooled_s, Cs, Cs), B, fs, params, False, None).materialise(B)
-    img, bias, widths = ops.pointnet_fused_image(_conv_layers(conv_g, params), F, bf16=ops.EVAL_BF16[0])
-    Ct = conv_g[-1].cout
-    G = 0 if glob is None else glob.shape[1]
-    ldp = _round4(Ct + G)
-    pooled = torch.empty((B, ldp), dtype=torch.float32, device=dev)
-    ops.pointnet_fused_eval(clouds, T, img, bias, widths, pooled, ldp)
-    if G > 0:
-        ops.affine_act(glob.contiguous(), G, B, G, out=pooled[:, Ct:], ldo=ldp)
-    return chain_forward(Deferred(pooled, ldp, Ct + G), B, fc_g, params, False, None).materialise(B)
-
-
-class _PointNetRaggedFunction(torch.autograd.Function):
-    """PointNet over CSR segments: the dense chains of _PointNetFunction with segmax_csr_* /
-    rows_xy_transform* in place of the constant-L kernels."""
-
-    @staticmethod
-    def forward(ctx, points, offsets, glob, nfeat_stn, groups, training, *params):
-        stn_g, conv_g, fc_g = groups
-        if points.dtype != torch.float32 or points.dim() != 2:
-            raise TypeError("ragged PointNet input must be float32 [P, nfeat]")
-        offsets = offsets.to(torch.int64).contiguous()
-        P, F = points.shape
-        B = offsets.numel() - 1
-        ld = _row_ld(F)
-        rows0 = torch.empty((P, ld), dtype=torch.float32, device=points.device)
-        ops.zero_(rows0)
-        ops.affine_act(points.contiguous(), F, P, F, out=rows0, ldo=ld)
-        row_seg = torch.repeat_interleave(torch.arange(B, device=points.device, dtype=torch.int32),
-                                          (offsets[1:] - offsets[:-1]))
-        saved = {} if training else None
-        T = None
-        rows = rows0
-        if nfeat_stn > 0:
-            cs, fs = stn_g
-            sv_c = [] if training else None
-            o = chain_forward(Deferred(rows0, ld, cs[0].cin), P, cs, params, training, sv_c)
-            Cs = o.C
-            pooled_s = torch.empty((B, Cs), dtype=torch.float32, device=points.device)
-            am_s = ops.segmax_csr_fwd(o.raw, o.ld, offsets, Cs, o.scale, o.shift, o.relu, pooled_s, Cs)
-            sv_f = [] if training else None
-            t = chain_forward(Deferred(pooled_s, Cs, Cs), B, fs, params, training, sv_f)
-            T = t.materialise(B)
-            rows = ops.rows_xy_transform(rows0, T, row_seg, add_eye=True)
-            if training:
-                saved.update(stn_c=sv_c, stn_f=sv_f, stn_am=am_s, stn_Cs=Cs)
-        sv_c = [] if training else None
-        out = chain_forward(Deferred(rows, ld, F), P, conv_g, params, training, sv_c)
-        Ct = out.C
-        G = 0 if glob is None else glob.shape[1]
-        ldp = _round4(Ct + G)
-        pooled = torch.empty((B, ldp), dtype=torch.float32, device=points.device)
-        am = ops.segmax_csr_fwd(out.raw, out.ld, offsets, Ct, out.scale, out.shift, out.relu, pooled, ldp)
-        if G > 0:
-            ops.affine_act(glob.contiguous(), G, B, G, out=pooled[:, Ct:], ldo=ldp)
-        sv_f = [] if training else None
-        y = chain_forward(Deferred(pooled, ldp, Ct + G), B, fc_g, params, training, sv_f)
-        res = y.materialise(B)
-        if training:
-            saved.update(conv=sv_c, fc=sv_f, am=am, Ct=Ct)
-        ctx.saved, ctx.groups, ctx.params = saved, groups, params
-        ctx.dims = (B, P, nfeat_stn)
-        ctx.aux = (offsets, rows0) if (training and nfeat_stn > 0) else None
-        return res
-
-    @staticmethod
-    def backward(ctx, gy):
-        if ctx.saved is None:
-            raise RuntimeError("backward through an eval-mode forward is not supported")
-        stn_g, conv_g, fc_g = ctx.groups
-        params, saved = ctx.params, ctx.saved
-        B, P, nfeat_stn = ctx.dims
-        grads = [None] * len(params)
-        Ct = saved["Ct"]
-        g_pool = chain_backward(gy.contiguous(), gy.shape[1], B, fc_g, params, saved["fc"], True, grads)
-        G = ops.segmax_csr_bwd(g_pool, g_pool.shape[1], saved["am"], P, Ct)
-        g_rows = chain_backward(G, Ct, P, conv_g, params, saved["conv"], nfeat_stn > 0, grads, own_g=True)
-        if nfeat_stn > 0:
-            offsets, rows0 = ctx.aux
-            cs, fs = stn_g
-            dT = ops.rows_xy_transform_bwd(rows0, g_rows, offsets)
-            g_ps = chain_backward(dT, 4, B, fs, params, saved["stn_f"], True, grads)
-            Gs = ops.segmax_csr_bwd(g_ps, g_ps.shape[1], saved["stn_am"], P, saved["stn_Cs"])
-            chain_backward(Gs, saved["stn_Cs"], P, cs, params, saved["stn_c"], False, grads, own_g=True)
-        ctx.saved = ctx.aux = None
-        return (None, None, None, None, None, None) + tuple(grads)
+            _stn_backward(layout, dT, stn_g, params, saved, grads)
+        elif want_input:  # external transformer (LocalCloudEmbedder): hand the gradient back as [B, F, L]
+            g_input = layout.input_grad(g_rows)
+        ctx.saved = ctx.layout = None
+        return (g_input, None, g_glob, None, None, None) + tuple(grads)
 
 
 class CloudEmbedder():

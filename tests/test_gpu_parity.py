@@ -373,7 +373,8 @@ def test_pointnet_small_golden(golden_dir, dev):
 def test_pointnet_ragged_csr(golden_dir, dev):
     """PointNet.forward_ragged (CSR offset array, no resample-to-ptn_npts): (1) with equal segment lengths
     it reproduces the reference's golden outputs and gradients; (2) with unequal lengths (1..300 points)
-    it matches the oracle's ragged restatement, forward and backward, S3DIS widths."""
+    it matches the oracle's ragged restatement, forward and backward (incl. the gradient w.r.t. the
+    global input), S3DIS widths."""
     from superpoint_graph_b200.spg_pointnet import PointNet
     g = load(golden_dir, "pointnet_small.npz")
     cfg = json.loads(str(g["cfg"]))
@@ -405,14 +406,17 @@ def test_pointnet_ragged_csr(golden_dir, dev):
     P = int(offsets[-1])
     points = torch.randn(P, 14) * 0.4
     glob = torch.rand(97) * 3
+    glob_ref, glob_dev = glob.clone().requires_grad_(True), glob.to(dev).requires_grad_(True)
     pcfg = dict(n_conv=5, n_fc=3, n_conv_stn=3, n_fc_stn=2, nfeat_stn=14)
-    ref = nets_ref.pointnet_forward_ragged(points, offsets, glob, sd, pcfg, True)
+    ref = nets_ref.pointnet_forward_ragged(points, offsets, glob_ref, sd, pcfg, True)
     gy = torch.randn(97, 32)
     ref.backward(gy)
     net.to(dev).train()
-    out = net.forward_ragged(points.to(dev), torch.from_numpy(offsets).to(dev), glob.to(dev))
+    out = net.forward_ragged(points.to(dev), torch.from_numpy(offsets).to(dev), glob_dev)
     close(out, ref)
     out.backward(gy.to(dev))
+    assert glob_dev.grad is not None, "missing gradient for input_global"
+    close(glob_dev.grad, glob_ref.grad, 1e-3)
     # (float32 oracle, BatchNorm over 1.5e4 points, max-pool ties: see tests/test_gpu_shapes.py's docstring)
     close_grads({k: p.grad for k, p in net.named_parameters()},
                 {k: v.grad for k, v in sd.items() if v.requires_grad}, 3e-2)
