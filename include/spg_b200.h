@@ -288,6 +288,33 @@ int spg_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                       const float* s2, float* dY, int64_t lddy, int64_t M, int C,
                       spg_stream_t stream);
 
+/* ------------------------------------------------------------ dropout     */
+/* Training-mode nn.Dropout(p) directly after a layer's [BatchNorm][ReLU] (ref: learning/pointnet.py:
+ * 109-110, learning/graphnet.py:54-55).  Element (m, c) of an [M, C] activation, i = m*C + c, is kept iff
+ * word i&3 of Philox4x32-10(counter = (i>>2 low 32 bits, i>>34, ctr_lo, ctr_hi), key = (seed_lo,
+ * seed_hi)) is >= floor(p * 2^32); kept elements are scaled by 1/(1-p); p >= 1 drops every element.  The
+ * mask depends on (seed, ctr, i) only; it is its own stream, not the bits of the reference's nn.Dropout.
+ * `slot` is an int64[2] (seed, ctr) in device memory.                                                  */
+/* slot = (state[0] ^ key_xor, state[1]); state[1] += 1.  state: the device's int64[2] (seed, counter);
+ * key_xor folds a data-parallel rank into the key (0 on one GPU).                                     */
+int spg_dropout_rng_next(int64_t* state, int64_t* slot, int64_t key_xor, spg_stream_t stream);
+/* out[m,c] = dropout(f(Y[m,c]*scale[c]+shift[c])), f = ReLU if relu; scale/shift may be NULL.          */
+int spg_dropout_fwd(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu, float p,
+                    const int64_t* slot, float* out, int64_t ldo, int64_t M, int C, spg_stream_t stream);
+/* mask[m*C+c] = 1 if element (m, c) is kept, else 0 (uint8, [M, C] contiguous).                       */
+int spg_dropout_mask(const int64_t* slot, float p, int64_t M, int C, uint8_t* mask, spg_stream_t stream);
+/* spg_act_bwd_reduce / spg_act_bwd_apply with the incoming gradient G (w.r.t. the dropped activation)
+ * first turned into G*m/(1-p), m regenerated from `slot`.  s12 = [s1 | s2] (2*C floats);
+ * workspace >= 2*C*spg_colstats_chunks(M) floats.  In apply, Y may be NULL without relu and BN.       */
+int spg_dropout_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy, const float* scale,
+                           const float* shift, const float* mean, const float* var, float eps, int relu, float p,
+                           const int64_t* slot, float* s12, float* workspace, int64_t M, int C,
+                           spg_stream_t stream);
+int spg_dropout_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy, const float* scale,
+                          const float* shift, const float* mean, const float* var, float eps, int relu, int has_bn,
+                          const float* s1, const float* s2, float p, const int64_t* slot, float* dY, int64_t lddy,
+                          int64_t M, int C, spg_stream_t stream);
+
 /* ------------------------------------------------------------ PointNet    */
 /* clouds [B,F,L] (the reference's NCL layout, learning/spg.py:162) -> rows [B*L, ld]
  * (point-major, channel contiguous, zero padded to ld).  If T [B,2,2] is given the

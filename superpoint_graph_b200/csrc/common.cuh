@@ -50,6 +50,12 @@ enum KernelId {
     K_TC_MERGE,
     K_POINTNET_FUSED,
     K_GRAPH_BUILD,
+    K_DROPOUT_RNG_NEXT,
+    K_DROPOUT_FWD,
+    K_DROPOUT_MASK,
+    K_DROPOUT_BWD_REDUCE,
+    K_DROPOUT_BWD_REDUCE_FINAL,
+    K_DROPOUT_BWD_APPLY,
     K_COUNT
 };
 

@@ -21,6 +21,8 @@ static const char* kKernelNames[K_COUNT] = {
     "tc_pack_weights",     "tc_dw_3xtf32",       "rnn_ecc_gru_fwd",     "rnn_ecc_gru_bwd",
     "cloud_build",       "confusion_count",    "tc_merge",
     "pointnet_fused_eval", "graph_build",
+    "dropout_rng_next",  "dropout_fwd",        "dropout_mask",        "dropout_bwd_reduce",
+    "dropout_bwd_reduce_final", "dropout_bwd_apply",
 };
 
 struct Record {

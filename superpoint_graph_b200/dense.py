@@ -19,18 +19,23 @@ from . import ops
 class LayerSpec(object):
     """One parametric layer: names index into the flat parameter list given to the chain."""
 
-    __slots__ = ("w", "b", "gamma", "beta", "bn", "relu", "cin", "cout")
+    __slots__ = ("w", "b", "gamma", "beta", "bn", "relu", "cin", "cout", "drop")
 
-    def __init__(self, w, b, gamma, beta, bn, relu, cin, cout):
+    def __init__(self, w, b, gamma, beta, bn, relu, cin, cout, drop=0.0):
         self.w, self.b, self.gamma, self.beta = w, b, gamma, beta
         self.bn, self.relu, self.cin, self.cout = bn, relu, cin, cout
+        self.drop = drop  # training-mode dropout probability applied after [BatchNorm][ReLU] (0: none)
 
 
 def parse_sequential(seq, training, params=None):
     """nn.Sequential -> ([LayerSpec], [parameter tensors]).  LayerSpec.w/b/gamma/beta are
     positions in the returned parameter list; LayerSpec.bn is the BatchNorm module (buffers).
     With `params` given, the parameters are appended to that list (and it is returned), so that
-    several chains index one flat list."""
+    several chains index one flat list.
+
+    A training-mode nn.Dropout(p > 0) is accepted directly after a layer's [BatchNorm1d][ReLU] and
+    recorded as that layer's `drop`; in eval mode, or with p = 0, dropout is the identity and leaves
+    no trace in the specs."""
     specs = []
     params = [] if params is None else params
     mods = list(seq.children()) if isinstance(seq, nn.Sequential) else list(seq)
@@ -46,8 +51,8 @@ def parse_sequential(seq, training, params=None):
         elif isinstance(m, nn.Dropout):
             if training and m.p > 0:
                 raise NotImplementedError(
-                    "dropout with p>0 in training mode is not implemented by the fused path "
-                    "(the reference's documented configs use ptn_prelast_do=0)")
+                    "training-mode dropout is supported only directly after a layer's activation, in the "
+                    "order Linear|Conv1d, [BatchNorm1d], [ReLU], Dropout (got %r at position %d)" % (m, i))
             i += 1
             continue
         else:
@@ -73,18 +78,26 @@ def parse_sequential(seq, training, params=None):
         if i < len(mods) and isinstance(mods[i], nn.ReLU):
             relu = True
             i += 1
-        specs.append(LayerSpec(w, b, gamma, beta, bn, relu, cin, cout))
+        drop = 0.0
+        if i < len(mods) and isinstance(mods[i], nn.Dropout):
+            if training and mods[i].p > 0:
+                drop = float(mods[i].p)
+            i += 1
+        specs.append(LayerSpec(w, b, gamma, beta, bn, relu, cin, cout, drop))
     return specs, params
 
 
 class Deferred(object):
-    """A raw activation [M, C] (leading dimension ld) plus the affine+ReLU still to be applied."""
+    """A raw activation [M, C] (leading dimension ld) plus the affine+ReLU still to be applied.
+    `drop` = (p, slot) on a layer's record when its activation went through training-mode dropout
+    (the consumer then reads the materialised dropped activation, never this record)."""
 
-    __slots__ = ("raw", "ld", "C", "scale", "shift", "relu")
+    __slots__ = ("raw", "ld", "C", "scale", "shift", "relu", "drop")
 
     def __init__(self, raw, ld, C, scale=None, shift=None, relu=False):
         self.raw, self.ld, self.C = raw, ld, C
         self.scale, self.shift, self.relu = scale, shift, relu
+        self.drop = None
 
     @property
     def pending(self):
@@ -162,10 +175,16 @@ def chain_forward(inp, M, specs, params, training, saved=None):
             else:
                 mean, var = bn.running_mean, bn.running_var
                 scale, shift = ops.bn_fold(mean, var, gamma, beta, bn.eps)
-        nxt = Deferred(y, sp.cout, sp.cout, scale, shift, sp.relu)
+        nxt = act = Deferred(y, sp.cout, sp.cout, scale, shift, sp.relu)
+        if sp.drop > 0 and training:
+            # dropout cannot ride in a GEMM prologue: BatchNorm-apply, ReLU and the mask in one pass, and
+            # the consumer (next layer's GEMM and weight gradient) reads the dropped activation as is
+            nxt.drop = (sp.drop, ops.dropout_slot(y.device))
+            act = Deferred(ops.dropout_fwd(y, sp.cout, M, sp.cout, scale, shift, sp.relu, sp.drop, nxt.drop[1]),
+                           sp.cout, sp.cout)
         if saved is not None:
             saved.append((cur, nxt, mean, var))
-        cur = nxt
+        cur = act
     return cur
 
 
@@ -183,7 +202,12 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
     around it is fused into that ONE launch: the prologue turns dL/d(activation) into dL/dY on the
     fly (and stores it once for the weight-gradient kernel), the epilogue reduces the BatchNorm-
     backward sums of the layer below from the tile it has just produced.  The stand-alone
-    act_bwd_reduce / act_bwd_apply kernels remain for the small-row chains."""
+    act_bwd_reduce / act_bwd_apply kernels remain for the small-row chains.
+
+    A layer with dropout masks the incoming gradient inside its own BatchNorm/ReLU backward
+    (dropout_bwd_reduce / dropout_bwd_apply, the mask regenerated from the forward's slot); both fused
+    paths that would read that gradient unmasked are off for it: the lazy prologue of its data-gradient
+    GEMM and the epilogue sums of the GEMM of the layer above."""
     red = None  # s1|s2 of the current layer, if the GEMM that produced G already reduced them
     for li in range(len(specs) - 1, -1, -1):
         sp = specs[li]
@@ -191,8 +215,9 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
         C = sp.cout
         Wp = params[sp.w]
         want_dx = li > 0 or need_input_grad
+        drop = nxt.drop  # (p, slot) if the activation of this layer went through dropout
         fused_pool = (pooled is not None and li == len(specs) - 1 and sp.bn is not None
-                      and mean is not None and C % 4 == 0)
+                      and mean is not None and C % 4 == 0 and drop is None)
         if G is None and not fused_pool:  # generic path: materialise the dense pooled gradient
             gp, ldgp, argmax, Bc, Lc = pooled
             G, ldg, own_g = ops.segmax_bwd(gp, ldgp, argmax, Bc, Lc, C), C, True
@@ -208,19 +233,33 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
                 grads[sp.beta] = s1
         elif sp.bn is not None:
             eps = sp.bn.eps
-            s12 = red if red is not None else ops.act_bwd_reduce(
-                G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps, nxt.relu, M, C)
+            if drop is not None:
+                assert red is None  # the layer above never reduces for a dropout layer (see bnred)
+                s12 = ops.dropout_bwd_reduce(G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps,
+                                             nxt.relu, drop[0], drop[1], M, C)
+            else:
+                s12 = red if red is not None else ops.act_bwd_reduce(
+                    G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps, nxt.relu, M, C)
             s1, s2 = s12[:C], s12[C:]
             if sp.gamma is not None:
                 grads[sp.gamma] = s2
                 grads[sp.beta] = s1
             if (ops.USE_FUSED_BNBWD[0] and want_dx and ldg % 4 == 0 and nxt.ld % 4 == 0 and mean is not None
-                    and ops.tc_supported(M, sp.cin, sp.cout, ldg, sp.cin)):
+                    and drop is None and ops.tc_supported(M, sp.cin, sp.cout, ldg, sp.cin)):
                 lazy = (nxt.raw, nxt.ld, nxt.scale, nxt.shift, nxt.relu, mean, var, s12, eps, True)
+            elif drop is not None:
+                out = G if (own_g and ldg == C) else None
+                dY = ops.dropout_bwd_apply(G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps,
+                                           nxt.relu, True, s1, s2, drop[0], drop[1], M, C, out=out, ldo=C)
             else:
                 out = G if (own_g and ldg == C) else None
                 dY = ops.act_bwd_apply(G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps,
                                        nxt.relu, True, s1, s2, M, C, out=out, ldo=C)
+        elif drop is not None:
+            out = G if (own_g and ldg == C) else None
+            dY = ops.dropout_bwd_apply(G, ldg, nxt.raw if sp.relu else None, nxt.ld, nxt.scale, nxt.shift, None,
+                                       None, 0.0, sp.relu, False, None, None, drop[0], drop[1], M, C,
+                                       out=out, ldo=C)
         elif sp.relu:
             out = G if (own_g and ldg == C) else None
             dY = ops.act_bwd_apply(G, ldg, nxt.raw, nxt.ld, None, None, None, None, 0.0, True,
@@ -274,7 +313,7 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
             if lazy is not None or ops.tc_supported(M, sp.cin, sp.cout, ldy, sp.cin):
                 bnred = None
                 if (ops.USE_FUSED_BNBWD[0] and li > 0 and specs[li - 1].bn is not None
-                        and saved[li - 1][2] is not None and cur.ld % 4 == 0):
+                        and saved[li - 1][2] is not None and saved[li - 1][1].drop is None and cur.ld % 4 == 0):
                     # `cur` is the layer below's deferred output: its raw y, BatchNorm fold and ReLU
                     bnred = (cur.raw, cur.ld, cur.scale, cur.shift, saved[li - 1][2], saved[li - 1][3],
                              specs[li - 1].bn.eps, cur.relu)

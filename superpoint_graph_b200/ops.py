@@ -570,6 +570,96 @@ def act_bwd_apply(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1
     return out
 
 
+# -------------------------------------------------------------------------- dropout
+_DROPOUT_RNG = {}  # device index -> int64[2] (seed, counter) on that device
+DROPOUT_KEY_XOR = {}  # device index -> value folded into the key (data-parallel rank, see Trainer)
+
+
+def _device(device):
+    if device is None:
+        return torch.device("cuda", torch.cuda.current_device())
+    device = torch.device(device)
+    return torch.device("cuda", device.index if device.index is not None else torch.cuda.current_device())
+
+
+def dropout_rng_state(device=None, create=True):
+    """The device's dropout generator state, an int64[2] (seed, counter) tensor that the kernels read and
+    advance.  Created on first use with a seed drawn from torch's default generator (so torch.manual_seed
+    makes runs reproducible) and counter 0; with create=False, None if it does not exist yet."""
+    dev = _device(device)
+    st = _DROPOUT_RNG.get(dev.index)
+    if st is None and create:
+        seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64))
+        st = torch.tensor([seed, 0], dtype=torch.int64).to(dev)
+        _DROPOUT_RNG[dev.index] = st
+    return st
+
+
+def _int64(v):
+    v = int(v) & (2 ** 64 - 1)
+    return v - 2 ** 64 if v >= 2 ** 63 else v
+
+
+def dropout_manual_seed(seed, device=None):
+    """Resets the device's dropout generator to (seed, counter 0)."""
+    dev = _device(device)
+    st = _DROPOUT_RNG.get(dev.index)
+    if st is None:
+        _DROPOUT_RNG[dev.index] = torch.tensor([_int64(seed), 0], dtype=torch.int64).to(dev)
+    else:
+        st[0].fill_(_int64(seed))
+        st[1].zero_()
+
+
+def dropout_slot(device):
+    """Takes the next counter of the device's generator: returns a fresh int64[2] slot (seed ^ key fold,
+    counter) in device memory, filled on the current stream (spg_dropout_rng_next)."""
+    dev = _device(device)
+    st = dropout_rng_state(dev)
+    slot = torch.empty(2, dtype=torch.int64, device=dev)
+    _lib.call("spg_dropout_rng_next", st, slot, _int64(DROPOUT_KEY_XOR.get(dev.index, 0)), _lib.current_stream())
+    return slot
+
+
+def dropout_fwd(Y, ldy, M, C, scale, shift, relu, p, slot):
+    """dropout(relu?(Y*scale+shift)) -> [M, C], mask from `slot`."""
+    _need_cuda(Y, slot)
+    out = torch.empty((M, C), dtype=torch.float32, device=Y.device)
+    _lib.call("spg_dropout_fwd", Y, ldy, scale, shift, int(bool(relu)), float(p), slot, out, C, M, C,
+              _lib.current_stream())
+    return out
+
+
+def dropout_mask(slot, p, M, C):
+    """uint8 [M, C] keep mask of (slot = (seed, ctr), p)."""
+    _need_cuda(slot)
+    mask = torch.empty((M, C), dtype=torch.uint8, device=slot.device)
+    _lib.call("spg_dropout_mask", _c(slot), float(p), M, C, mask, _lib.current_stream())
+    return mask
+
+
+def dropout_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, p, slot, M, C):
+    """act_bwd_reduce of the gradient G*m/(1-p) -> s12 [2C]."""
+    _need_cuda(G, Y, slot)
+    s12 = torch.empty(2 * C, dtype=torch.float32, device=G.device)
+    ws = workspace(2 * C * _chunks(M), G.device)
+    _lib.call("spg_dropout_bwd_reduce", G, ldg, Y, ldy, scale, shift, mean, var, float(eps), int(bool(relu)),
+              float(p), slot, s12, ws, M, C, _lib.current_stream())
+    return s12
+
+
+def dropout_bwd_apply(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, p, slot, M, C,
+                      out=None, ldo=None):
+    """act_bwd_apply of the gradient G*m/(1-p) -> dY [M, C]."""
+    _need_cuda(G, slot)
+    if out is None:
+        out = torch.empty((M, C), dtype=torch.float32, device=G.device)
+        ldo = C
+    _lib.call("spg_dropout_bwd_apply", G, ldg, Y, ldy, scale, shift, mean, var, float(eps), int(bool(relu)),
+              int(bool(has_bn)), s1, s2, float(p), slot, out, ldo, M, C, _lib.current_stream())
+    return out
+
+
 # ------------------------------------------------------------------------- PointNet
 def cloud_rows(clouds, T, ld, add_eye=False):
     _need_cuda(clouds, T)

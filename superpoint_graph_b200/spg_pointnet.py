@@ -481,14 +481,26 @@ class CloudEmbedder():
     def _embed_monger(self, model, clouds, clouds_global, idx_valid, n_rows):
         """Memory mongering (ref: learning/pointnet.py:160-180): forward without saving, full
         recomputation in `bw_hook`.  As in the reference, a training step therefore runs the
-        training-mode forward twice and the BatchNorm running statistics see two updates."""
+        training-mode forward twice and the BatchNorm running statistics see two updates.  Unlike the
+        reference, the recomputation reuses the forward's dropout masks (the device counter is rewound to
+        its value before the forward, then restored), so the gradient is the true gradient of the
+        forward whose output was used."""
         was_training = model.training
+        rng = None
+        if was_training and any(isinstance(m, nn.Dropout) and m.p > 0 for m in model.ptn.modules()):
+            rng = ops.dropout_rng_state(clouds.device)
+            ctr0 = rng[1].clone()
         with torch.no_grad():
             out = model.ptn(clouds, clouds_global)
         out = out.detach().requires_grad_(was_training)
 
         def bw_hook():
+            if rng is not None:
+                ctr1 = rng[1].clone()
+                rng[1].copy_(ctr0)
             out_v2 = model.ptn(clouds, clouds_global)
+            if rng is not None:
+                rng[1].copy_(ctr1)
             out_v2.backward(out.grad)
 
         self.bw_hook = bw_hook

@@ -141,6 +141,9 @@ class Trainer(object):
         self._fused_ar = None
         if world_size > 1:  # one-time setup collective: guarantee identical replicas
             torch.distributed.broadcast(self.flat, 0, group=process_group)
+            if self.flat.is_cuda:  # every rank draws its own dropout masks: the rank is folded into the key
+                rank = torch.distributed.get_rank(process_group)
+                ops.DROPOUT_KEY_XOR[self.flat.device.index] = rank * 0x9E3779B97F4A7C15
             if self.flat.is_cuda and ops.USE_FUSED_ALLREDUCE[0]:
                 # gradient buffer in symmetric memory: all-reduce + clamp + Adam become ONE kernel over
                 # NVLink peer pointers; any failure to set that up leaves the NCCL path in place
@@ -242,11 +245,19 @@ class Trainer(object):
     # captured).  Batches of new shapes simply run eagerly.
     def _snapshot(self):
         bufs = [b for b in self.model.buffers()]
+        rng = ops.dropout_rng_state(self.flat.device, create=False) if self.flat.is_cuda else None
         return (self.flat.clone(), self.exp_avg.clone(), self.exp_avg_sq.clone(), self.step_dev.clone(),
-                self.step_count, bufs, [b.clone() for b in bufs])
+                self.step_count, bufs, [b.clone() for b in bufs], None if rng is None else rng.clone())
 
     def _restore(self, snap):
-        flat, m, v, step_dev, step_count, bufs, saved = snap
+        flat, m, v, step_dev, step_count, bufs, saved, rng = snap
+        # dropout generator: back to the snapshot's (seed, counter); one that the steps in between created
+        # (first use draws the seed) keeps its seed and restarts at counter 0, as a first step would
+        cur = ops.dropout_rng_state(self.flat.device, create=False) if self.flat.is_cuda else None
+        if rng is not None:
+            cur.copy_(rng)
+        elif cur is not None:
+            cur[1].zero_()
         self.flat.copy_(flat)
         self.exp_avg.copy_(m)
         self.exp_avg_sq.copy_(v)
@@ -258,8 +269,8 @@ class Trainer(object):
     def capture(self, db, key=None, warmup=2):
         """Captures compute_gradients on the static tensors of `db`; returns the key for replay().
         Free of side effects: the `warmup` (>= 1) eager steps that prime workspaces, weight-image
-        tables and lazy handles run on a snapshot — parameters, Adam state, step count and BatchNorm
-        buffers are restored before the capture."""
+        tables and lazy handles run on a snapshot — parameters, Adam state, step count, BatchNorm
+        buffers and the dropout generator are restored before the capture."""
         if warmup < 1:
             raise ValueError("capture() needs at least one warm-up step (the batched weight packing uploads "
                              "its job table on first use, which cannot happen inside a capture)")
