@@ -266,27 +266,33 @@ int spg_bn_fold(const float* mean, const float* var, const float* gamma, const f
                 float eps, float* scale, float* shift, float* running_mean, float* running_var,
                 int64_t* num_batches_tracked, float momentum, int64_t M, int C,
                 spg_stream_t stream);
-/* out[m,c] = f(Y[m,c]*scale[c]+shift[c]); scale/shift may be NULL.               */
+/* out[m,c] = drop(f(Y[m,c]*scale[c]+shift[c])); scale/shift may be NULL; drop: see below. */
 int spg_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                   float* out, int64_t ldo, int64_t M, int C, spg_stream_t stream);
+                   float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* drop_slot,
+                   spg_stream_t stream);
 /* Column sums: out[c] = sum_m X[m,c]; workspace >= C*spg_colstats_chunks(M).      */
 int spg_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float* workspace,
                spg_stream_t stream);
-/* Backward of a = relu?(bn?(y)):
- *   pass 1 (spg_act_bwd_reduce, BN layers only):
- *       s1[c] = sum_m G*mask, s2[c] = sum_m G*mask*xhat       (= d_beta, d_gamma)
- *   pass 2 (spg_act_bwd_apply): dY = scale*(G*mask - s1/M - xhat*s2/M)   (BN)
- *                               dY = G*mask                             (no BN)
- *   mask = (y*scale+shift > 0) if relu else 1; xhat = (y-mean)*rstd; in-place OK. */
+/* Backward of a = drop(relu?(bn?(y))):
+ *   pass 1 (spg_act_bwd_reduce, BN layers only): s12 = [s1 | s2] (2*C floats),
+ *       s1[c] = sum_m g*mask, s2[c] = sum_m g*mask*xhat       (= d_beta, d_gamma)
+ *       workspace >= 2*C*spg_colstats_chunks(M) floats
+ *   pass 2 (spg_act_bwd_apply): dY = scale*(g*mask - s1/M - xhat*s2/M)   (BN)
+ *                               dY = g*mask                             (no BN)
+ *   g = drop'(G); mask = (y*scale+shift > 0) if relu else 1; xhat = (y-mean)*rstd; in-place OK;
+ *   in apply, Y may be NULL without relu and BN.
+ * drop: with drop_slot == NULL the identity (p ignored); otherwise training-mode dropout with the mask of
+ * `drop_slot` (below): drop(a) = a*m/(1-p) and drop'(G) = G*m/(1-p), as a select, so that p >= 1 or an
+ * infinite G gives 0.                                                                              */
 int spg_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                        const float* scale, const float* shift, const float* mean,
-                       const float* var, float eps, int relu, float* s1, float* s2,
-                       float* workspace, int64_t M, int C, spg_stream_t stream);
+                       const float* var, float eps, int relu, float* s12, float* workspace,
+                       int64_t M, int C, float p, const int64_t* drop_slot, spg_stream_t stream);
 int spg_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                       const float* scale, const float* shift, const float* mean,
                       const float* var, float eps, int relu, int has_bn, const float* s1,
-                      const float* s2, float* dY, int64_t lddy, int64_t M, int C,
-                      spg_stream_t stream);
+                      const float* s2, float* dY, int64_t lddy, int64_t M, int C, float p,
+                      const int64_t* drop_slot, spg_stream_t stream);
 
 /* ------------------------------------------------------------ dropout     */
 /* Training-mode nn.Dropout(p) directly after a layer's [BatchNorm][ReLU] (ref: learning/pointnet.py:
@@ -294,26 +300,13 @@ int spg_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
  * word i&3 of Philox4x32-10(counter = (i>>2 low 32 bits, i>>34, ctr_lo, ctr_hi), key = (seed_lo,
  * seed_hi)) is >= floor(p * 2^32); kept elements are scaled by 1/(1-p); p >= 1 drops every element.  The
  * mask depends on (seed, ctr, i) only; it is its own stream, not the bits of the reference's nn.Dropout.
- * `slot` is an int64[2] (seed, ctr) in device memory.                                                  */
+ * `slot` is an int64[2] (seed, ctr) in device memory.  The masked forward and backward are
+ * spg_affine_act / spg_act_bwd_reduce / spg_act_bwd_apply with a drop_slot.                           */
 /* slot = (state[0] ^ key_xor, state[1]); state[1] += 1.  state: the device's int64[2] (seed, counter);
  * key_xor folds a data-parallel rank into the key (0 on one GPU).                                     */
 int spg_dropout_rng_next(int64_t* state, int64_t* slot, int64_t key_xor, spg_stream_t stream);
-/* out[m,c] = dropout(f(Y[m,c]*scale[c]+shift[c])), f = ReLU if relu; scale/shift may be NULL.          */
-int spg_dropout_fwd(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu, float p,
-                    const int64_t* slot, float* out, int64_t ldo, int64_t M, int C, spg_stream_t stream);
 /* mask[m*C+c] = 1 if element (m, c) is kept, else 0 (uint8, [M, C] contiguous).                       */
 int spg_dropout_mask(const int64_t* slot, float p, int64_t M, int C, uint8_t* mask, spg_stream_t stream);
-/* spg_act_bwd_reduce / spg_act_bwd_apply with the incoming gradient G (w.r.t. the dropped activation)
- * first turned into G*m/(1-p), m regenerated from `slot`.  s12 = [s1 | s2] (2*C floats);
- * workspace >= 2*C*spg_colstats_chunks(M) floats.  In apply, Y may be NULL without relu and BN.       */
-int spg_dropout_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy, const float* scale,
-                           const float* shift, const float* mean, const float* var, float eps, int relu, float p,
-                           const int64_t* slot, float* s12, float* workspace, int64_t M, int C,
-                           spg_stream_t stream);
-int spg_dropout_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy, const float* scale,
-                          const float* shift, const float* mean, const float* var, float eps, int relu, int has_bn,
-                          const float* s1, const float* s2, float p, const int64_t* slot, float* dY, int64_t lddy,
-                          int64_t M, int C, spg_stream_t stream);
 
 /* ------------------------------------------------------------ PointNet    */
 /* clouds [B,F,L] (the reference's NCL layout, learning/spg.py:162) -> rows [B*L, ld]

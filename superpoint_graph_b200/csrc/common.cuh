@@ -87,19 +87,21 @@ __device__ __forceinline__ void st_stream4(float4* p, float4 v) { __stcs(p, v); 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.f / (1.f + expf(-v)); }
 
 // 128-bit vectorised variants (dense_vec.cu); return false if the shape/alignment does not fit.
+// slot != NULL: dropout with probability p (see spg_affine_act).
 bool vec_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                         const float* scale, const float* shift, const float* mean,
-                        const float* var, float eps, int relu, float* s1, float* s2, float* ws,
-                        int64_t M, int C, cudaStream_t s, int* rc);
+                        const float* var, float eps, int relu, float* s12, float* ws,
+                        int64_t M, int C, float p, const int64_t* slot, cudaStream_t s, int* rc);
 bool vec_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float* ws,
                 cudaStream_t s, int* rc);
 bool vec_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                        const float* scale, const float* shift, const float* mean,
                        const float* var, float eps, int relu, int has_bn, const float* s1,
-                       const float* s2, float* dY, int64_t lddy, int64_t M, int C,
-                       cudaStream_t s, int* rc);
+                       const float* s2, float* dY, int64_t lddy, int64_t M, int C, float p,
+                       const int64_t* slot, cudaStream_t s, int* rc);
 bool vec_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                    float* out, int64_t ldo, int64_t M, int C, cudaStream_t s, int* rc);
+                    float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* slot,
+                    cudaStream_t s, int* rc);
 
 }  // namespace spg
 

@@ -12,6 +12,7 @@
 // small / odd shapes).  The large point-wise layers are served by the wgmma
 // 3xTF32 kernel in tc_gemm.cu when it applies.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace spg {
 
@@ -332,6 +333,8 @@ gemm_splitk_reduce_kernel(const float* __restrict__ ws, int split, int64_t M, in
 
 // ---------------------------------------------------------------- column reductions
 constexpr int kChunkRows = 1024;
+// the masked BatchNorm-backward sums spend a Philox call per element: shorter chunks, more CTAs
+constexpr int kDropChunkRows = 256;
 
 // per (chunk, column): count, mean, M2 (Welford), merged over the 8 row lanes (Chan).
 __global__ void __launch_bounds__(256)
@@ -523,18 +526,22 @@ __global__ void bn_fold_kernel(const float* __restrict__ mean, const float* __re
     if (rvar) rvar[c] = (1.f - momentum) * rvar[c] + momentum * v * unbias;
 }
 
+// DROP (here and in the act_bwd kernels): dropout with probability p, mask from `slot` (philox.cuh)
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 affine_act_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
                   const float* __restrict__ shift, int relu, float* __restrict__ out, int64_t ldo,
-                  int64_t M, int C) {
+                  int64_t M, int C, float p, const int64_t* __restrict__ slot) {
     SPG_PDL_ENTRY();
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = blockIdx.x * 32 + x;
     if (c >= C) return;
     const float sc = scale ? scale[c] : 1.f, sh = shift ? shift[c] : 0.f;
+    const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
     for (int64_t r = (int64_t)blockIdx.y * 8 + y; r < M; r += (int64_t)gridDim.y * 8) {
         float v = fmaf(Y[r * ldy + c], sc, sh);
         if (relu) v = fmaxf(v, 0.f);
+        if constexpr (DROP) v = drop_at(d, r * C + c, v);
         out[r * ldo + c] = v;
     }
 }
@@ -571,25 +578,29 @@ __global__ void colsum_final_kernel(const float* __restrict__ ws, int64_t chunks
     out[c] = (float)a;
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 act_bwd_reduce_kernel(const float* __restrict__ G, int64_t ldg, const float* __restrict__ Y,
                       int64_t ldy, const float* __restrict__ scale,
                       const float* __restrict__ shift, const float* __restrict__ mean,
                       const float* __restrict__ var, float eps, int relu, float* __restrict__ ws,
-                      int64_t M, int C) {
+                      int64_t M, int C, float p, const int64_t* __restrict__ slot) {
     SPG_PDL_ENTRY();
     __shared__ float s1[8][32], s2[8][32];
+    constexpr int kRows = DROP ? kDropChunkRows : kChunkRows;
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = blockIdx.x * 32 + x;
-    const int64_t r0 = (int64_t)blockIdx.y * kChunkRows;
-    const int64_t r1 = min(M, r0 + kChunkRows);
+    const int64_t r0 = (int64_t)blockIdx.y * kRows;
+    const int64_t r1 = min(M, r0 + kRows);
     float a1 = 0.f, a2 = 0.f;
     if (c < C) {
         const float sc = scale[c], sh = shift[c], mu = mean[c];
         const float rstd = 1.f / sqrtf(var[c] + eps);
+        const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
         for (int64_t r = r0 + y; r < r1; r += 8) {
             const float yv = __ldg(Y + r * ldy + c);
             float g = __ldg(G + r * ldg + c);
+            if constexpr (DROP) g = drop_at(d, r * C + c, g);
             if (relu && !(fmaf(yv, sc, sh) > 0.f)) g = 0.f;
             a1 += g;
             a2 = fmaf(g, (yv - mu) * rstd, a2);
@@ -623,13 +634,14 @@ __global__ void act_bwd_reduce_final_kernel(const float* __restrict__ ws, int64_
     s2[c] = (float)a2;
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 act_bwd_apply_kernel(const float* __restrict__ G, int64_t ldg, const float* __restrict__ Y,
                      int64_t ldy, const float* __restrict__ scale, const float* __restrict__ shift,
                      const float* __restrict__ mean, const float* __restrict__ var, float eps,
                      int relu, int has_bn, const float* __restrict__ s1,
                      const float* __restrict__ s2, float* __restrict__ dY, int64_t lddy, int64_t M,
-                     int C) {
+                     int C, float p, const int64_t* __restrict__ slot) {
     SPG_PDL_ENTRY();
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = blockIdx.x * 32 + x;
@@ -643,9 +655,11 @@ act_bwd_apply_kernel(const float* __restrict__ G, int64_t ldg, const float* __re
         m1 = s1[c] / (float)M;
         m2 = s2[c] / (float)M;
     }
+    const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
     for (int64_t r = (int64_t)blockIdx.y * 8 + y; r < M; r += (int64_t)gridDim.y * 8) {
         const float yv = Y ? Y[r * ldy + c] : 0.f;
         float g = G[r * ldg + c];
+        if constexpr (DROP) g = drop_at(d, r * C + c, g);
         if (relu && !(fmaf(yv, sc, sh) > 0.f)) g = 0.f;
         float d = g;
         if (has_bn) d = sc * (g - m1 - (yv - mu) * rstd * m2);
@@ -791,26 +805,32 @@ int spg_bn_fold(const float* mean, const float* var, const float* gamma, const f
     return launch_status();
 }
 
-static inline unsigned rows_grid(int64_t M) {
-    int64_t g = ceil_div64(M, 64);
+// CTAs along the rows of the element-wise passes; the masked (DROP) passes are bound by the Philox
+// latency, not by bandwidth: one row step per thread where the cap allows.
+static inline unsigned rows_grid(int64_t M, bool drop) {
+    int64_t g = ceil_div64(M, drop ? 8 : 64);
     if (g > 8 * kNumSMs) g = 8 * kNumSMs;
     if (g < 1) g = 1;
     return (unsigned)g;
 }
 
 int spg_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                   float* out, int64_t ldo, int64_t M, int C, spg_stream_t stream) {
-    if (M < 0 || C <= 0) return SPG_E_BADARG;
+                   float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* drop_slot,
+                   spg_stream_t stream) {
+    if (M < 0 || C <= 0 || (drop_slot && !(p >= 0.f))) return SPG_E_BADARG;
     if (M == 0) return SPG_OK;
     if (!Y || !out || ldy < C || ldo < C) return SPG_E_BADARG;
     {
         int rc = 0;
-        if (vec_affine_act(Y, ldy, scale, shift, relu, out, ldo, M, C, (cudaStream_t)stream, &rc))
+        if (vec_affine_act(Y, ldy, scale, shift, relu, out, ldo, M, C, p, drop_slot,
+                           (cudaStream_t)stream, &rc))
             return rc;
     }
-    dim3 grid((unsigned)ceil_div64(C, 32), rows_grid(M));
-    SPG_LAUNCH(K_AFFINE_ACT, (cudaStream_t)stream, affine_act_kernel, grid, 256, 0, Y, ldy, scale,
-               shift, relu, out, ldo, M, C);
+    const bool drop = drop_slot != nullptr;
+    dim3 grid((unsigned)ceil_div64(C, 32), rows_grid(M, drop));
+    SPG_LAUNCH(drop ? K_DROPOUT_FWD : K_AFFINE_ACT, (cudaStream_t)stream,
+               (drop ? affine_act_kernel<true> : affine_act_kernel<false>), grid, 256, 0, Y, ldy,
+               scale, shift, relu, out, ldo, M, C, p, drop_slot);
     return launch_status();
 }
 
@@ -835,36 +855,39 @@ int spg_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float*
 
 int spg_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                        const float* scale, const float* shift, const float* mean,
-                       const float* var, float eps, int relu, float* s1, float* s2,
-                       float* workspace, int64_t M, int C, spg_stream_t stream) {
-    if (M <= 0 || C <= 0 || !G || !Y || !scale || !shift || !mean || !var || !s1 || !s2 ||
-        !workspace)
+                       const float* var, float eps, int relu, float* s12, float* workspace,
+                       int64_t M, int C, float p, const int64_t* drop_slot, spg_stream_t stream) {
+    if (M <= 0 || C <= 0 || !G || !Y || !scale || !shift || !mean || !var || !s12 ||
+        !workspace || (drop_slot && !(p >= 0.f)))
         return SPG_E_BADARG;
-    if (s2 == s1 + C) {
+    {
         int rc = 0;
-        if (vec_act_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, s1, s2,
-                               workspace, M, C, (cudaStream_t)stream, &rc))
+        if (vec_act_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, s12, workspace,
+                               M, C, p, drop_slot, (cudaStream_t)stream, &rc))
             return rc;
     }
-    const int64_t chunks = scalar_chunks(M);
+    const bool drop = drop_slot != nullptr;
+    const int64_t chunks = drop ? ceil_div64(M, kDropChunkRows) : scalar_chunks(M);
     if (chunks > 65535) return SPG_E_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)chunks);
-    SPG_LAUNCH(K_ACT_BWD_REDUCE, s, act_bwd_reduce_kernel, grid, 256, 0, G, ldg, Y, ldy, scale,
-               shift, mean, var, eps, relu, workspace, M, C);
+    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE : K_ACT_BWD_REDUCE, s,
+               (drop ? act_bwd_reduce_kernel<true> : act_bwd_reduce_kernel<false>), grid, 256, 0,
+               G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, workspace, M, C, p, drop_slot);
     int rc = launch_status();
     if (rc) return rc;
-    SPG_LAUNCH(K_ACT_BWD_REDUCE_FINAL, s, act_bwd_reduce_final_kernel,
-               (unsigned)ceil_div64(C, 128), 128, 0, workspace, chunks, C, s1, s2);
+    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE_FINAL : K_ACT_BWD_REDUCE_FINAL, s,
+               act_bwd_reduce_final_kernel, (unsigned)ceil_div64(C, 128), 128, 0, workspace, chunks,
+               C, s12, s12 + C);
     return launch_status();
 }
 
 int spg_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                       const float* scale, const float* shift, const float* mean,
                       const float* var, float eps, int relu, int has_bn, const float* s1,
-                      const float* s2, float* dY, int64_t lddy, int64_t M, int C,
-                      spg_stream_t stream) {
-    if (M < 0 || C <= 0) return SPG_E_BADARG;
+                      const float* s2, float* dY, int64_t lddy, int64_t M, int C, float p,
+                      const int64_t* drop_slot, spg_stream_t stream) {
+    if (M < 0 || C <= 0 || (drop_slot && !(p >= 0.f))) return SPG_E_BADARG;
     if (M == 0) return SPG_OK;
     if (!G || !dY) return SPG_E_BADARG;
     if ((relu || has_bn) && !Y) return SPG_E_BADARG;
@@ -872,12 +895,15 @@ int spg_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
     {
         int rc = 0;
         if (vec_act_bwd_apply(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2,
-                              dY, lddy, M, C, (cudaStream_t)stream, &rc))
+                              dY, lddy, M, C, p, drop_slot, (cudaStream_t)stream, &rc))
             return rc;
     }
-    dim3 grid((unsigned)ceil_div64(C, 32), rows_grid(M));
-    SPG_LAUNCH(K_ACT_BWD_APPLY, (cudaStream_t)stream, act_bwd_apply_kernel, grid, 256, 0, G, ldg, Y,
-               ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, dY, lddy, M, C);
+    const bool drop = drop_slot != nullptr;
+    dim3 grid((unsigned)ceil_div64(C, 32), rows_grid(M, drop));
+    SPG_LAUNCH(drop ? K_DROPOUT_BWD_APPLY : K_ACT_BWD_APPLY, (cudaStream_t)stream,
+               (drop ? act_bwd_apply_kernel<true> : act_bwd_apply_kernel<false>), grid, 256, 0, G,
+               ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, dY, lddy, M, C, p,
+               drop_slot);
     return launch_status();
 }
 

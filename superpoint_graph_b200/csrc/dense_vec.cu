@@ -3,7 +3,10 @@
 // for the PointNet / filter-network layers); dense.cu keeps the scalar kernels for odd shapes.
 // A warp covers 128 consecutive columns of one row (512 B), 8 row lanes per CTA, 256 rows per
 // CTA, 4 independent float4 loads in flight per thread and tensor.
+// DROP kernels apply dropout (philox.cuh): C % 4 == 0 and c % 4 == 0, so the float4 at (r, c) is
+// exactly the Philox group (r*C + c) >> 2 and its lane j uses word j.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace spg {
 
@@ -20,11 +23,14 @@ struct LaneMap {
     int rpw;   // rows per warp step
     int x, sub;
 };
+__host__ __device__ __forceinline__ int lanes_per_row(int C) {
+    const int q = C >> 2;
+    return (q < 32 && (q & (q - 1)) == 0) ? q : 32;
+}
 __device__ __forceinline__ LaneMap lane_map(int C) {
     LaneMap m;
     const int lane = threadIdx.x & 31;
-    const int q = C >> 2;
-    m.cpl = (q < 32 && (q & (q - 1)) == 0) ? q : 32;
+    m.cpl = lanes_per_row(C);
     m.rpw = 32 / m.cpl;
     m.x = lane % m.cpl;
     m.sub = lane / m.cpl;
@@ -40,12 +46,14 @@ __device__ __forceinline__ float4 fold_rows(float4 a, int cpl) {
     return a;
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 act_bwd_reduce_v4_kernel(const float* __restrict__ G, int64_t ldg, const float* __restrict__ Y,
                          int64_t ldy, const float* __restrict__ scale,
                          const float* __restrict__ shift, const float* __restrict__ mean,
                          const float* __restrict__ var, float eps, int relu,
-                         float* __restrict__ ws, int64_t M, int C) {
+                         float* __restrict__ ws, int64_t M, int C, float p,
+                         const int64_t* __restrict__ slot) {
     SPG_PDL_ENTRY();
     __shared__ float4 s1[8][32], s2[8][32];
     const LaneMap lm = lane_map(C);
@@ -61,10 +69,18 @@ act_bwd_reduce_v4_kernel(const float* __restrict__ G, int64_t ldg, const float* 
         const float4 vr = *reinterpret_cast<const float4*>(var + c);
         const float4 rs = make_float4(1.f / sqrtf(vr.x + eps), 1.f / sqrtf(vr.y + eps),
                                       1.f / sqrtf(vr.z + eps), 1.f / sqrtf(vr.w + eps));
+        const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
 #pragma unroll 4
         for (int64_t r = r0 + y * lm.rpw + lm.sub; r < r1; r += 8 * lm.rpw) {
             const float4 yv = __ldg(reinterpret_cast<const float4*>(Y + r * ldy + c));
             float4 g = __ldg(reinterpret_cast<const float4*>(G + r * ldg + c));
+            if constexpr (DROP) {
+                const Philox4 w = dropout_words(d.seed, d.ctr, (uint64_t)((r * C + c) >> 2));
+                g.x = drop1(d, w.v[0], g.x);
+                g.y = drop1(d, w.v[1], g.y);
+                g.z = drop1(d, w.v[2], g.z);
+                g.w = drop1(d, w.v[3], g.w);
+            }
             if (relu) {
                 if (!(fmaf(yv.x, sc.x, sh.x) > 0.f)) g.x = 0.f;
                 if (!(fmaf(yv.y, sc.y, sh.y) > 0.f)) g.y = 0.f;
@@ -142,13 +158,15 @@ colsum_merge_kernel(const float* __restrict__ ws, int64_t chunks, int C, float* 
     if (lane == 0) out[c] = (float)a;
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 act_bwd_apply_v4_kernel(const float* __restrict__ G, int64_t ldg, const float* __restrict__ Y,
                         int64_t ldy, const float* __restrict__ scale,
                         const float* __restrict__ shift, const float* __restrict__ mean,
                         const float* __restrict__ var, float eps, int relu, int has_bn,
                         const float* __restrict__ s1, const float* __restrict__ s2,
-                        float* __restrict__ dY, int64_t lddy, int64_t M, int C) {
+                        float* __restrict__ dY, int64_t lddy, int64_t M, int C, float p,
+                        const int64_t* __restrict__ slot) {
     SPG_PDL_ENTRY();
     const LaneMap lm = lane_map(C);
     const int x = lm.x, y = (threadIdx.x >> 5) * lm.rpw + lm.sub;
@@ -169,6 +187,7 @@ act_bwd_apply_v4_kernel(const float* __restrict__ G, int64_t ldg, const float* _
             m2[j] = s2[c + j] / (float)M;
         }
     }
+    const DropParams dp = DROP ? drop_params(slot, p) : DropParams{};
 #pragma unroll 4
     for (int64_t r = (int64_t)blockIdx.y * rows_per_block + y; r < M;
          r += (int64_t)gridDim.y * rows_per_block) {
@@ -177,6 +196,11 @@ act_bwd_apply_v4_kernel(const float* __restrict__ G, int64_t ldg, const float* _
         const float4 gq = __ldg(reinterpret_cast<const float4*>(G + r * ldg + c));
         const float yv[4] = {yq.x, yq.y, yq.z, yq.w};
         float g[4] = {gq.x, gq.y, gq.z, gq.w};
+        if constexpr (DROP) {
+            const Philox4 w = dropout_words(dp.seed, dp.ctr, (uint64_t)((r * C + c) >> 2));
+#pragma unroll
+            for (int j = 0; j < 4; ++j) g[j] = drop1(dp, w.v[j], g[j]);
+        }
         float d[4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -187,10 +211,11 @@ act_bwd_apply_v4_kernel(const float* __restrict__ G, int64_t ldg, const float* _
     }
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 affine_act_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
                      const float* __restrict__ shift, int relu, float* __restrict__ out,
-                     int64_t ldo, int64_t M, int C) {
+                     int64_t ldo, int64_t M, int C, float p, const int64_t* __restrict__ slot) {
     SPG_PDL_ENTRY();
     const LaneMap lm = lane_map(C);
     const int x = lm.x, y = (threadIdx.x >> 5) * lm.rpw + lm.sub;
@@ -203,6 +228,7 @@ affine_act_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __re
         if (scale) sc[j] = scale[c + j];
         if (shift) sh[j] = shift[c + j];
     }
+    const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
 #pragma unroll 4
     for (int64_t r = (int64_t)blockIdx.y * rows_per_block + y; r < M;
          r += (int64_t)gridDim.y * rows_per_block) {
@@ -213,6 +239,11 @@ affine_act_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __re
             v[j] = fmaf(v[j], sc[j], sh[j]);
             if (relu) v[j] = fmaxf(v[j], 0.f);
         }
+        if constexpr (DROP) {
+            const Philox4 w = dropout_words(d.seed, d.ctr, (uint64_t)((r * C + c) >> 2));
+#pragma unroll
+            for (int j = 0; j < 4; ++j) v[j] = drop1(d, w.v[j], v[j]);
+        }
         *reinterpret_cast<float4*>(out + r * ldo + c) = make_float4(v[0], v[1], v[2], v[3]);
     }
 }
@@ -220,31 +251,34 @@ affine_act_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __re
 static inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 static inline bool ld4(int64_t ld) { return (ld & 3) == 0; }
 
-static inline unsigned row_grid(int64_t M) {
-    int64_t g = ceil_div64(M, 32);
+// CTAs along the rows of the element-wise passes.  The masked (DROP) passes are bound by the Philox
+// latency, not by bandwidth: they get one row step per thread where the cap allows.
+static inline unsigned row_grid(int64_t M, int C, bool drop) {
+    int64_t g = ceil_div64(M, drop ? 8 * (32 / lanes_per_row(C)) : 32);
     if (g > 16 * kNumSMs) g = 16 * kNumSMs;
     return (unsigned)(g < 1 ? 1 : g);
 }
 
 bool vec_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                         const float* scale, const float* shift, const float* mean,
-                        const float* var, float eps, int relu, float* s1, float* s2, float* ws,
-                        int64_t M, int C, cudaStream_t s, int* rc) {
+                        const float* var, float eps, int relu, float* s12, float* ws,
+                        int64_t M, int C, float p, const int64_t* slot, cudaStream_t s, int* rc) {
     if ((C & 3) || !ld4(ldg) || !ld4(ldy) || !al16(G) || !al16(Y) || !al16(scale) ||
         !al16(shift) || !al16(mean) || !al16(var) || !al16(ws))
         return false;
     const int64_t chunks = ceil_div64(M, kVecRows);
     if (chunks > 65535) return false;
+    const bool drop = slot != nullptr;
     dim3 grid((unsigned)ceil_div64(C, 128), (unsigned)chunks);
-    SPG_LAUNCH(K_ACT_BWD_REDUCE, s, act_bwd_reduce_v4_kernel, grid, 256, 0, G, ldg, Y, ldy, scale,
-               shift, mean, var, eps, relu, ws, M, C);
+    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE : K_ACT_BWD_REDUCE, s,
+               (drop ? act_bwd_reduce_v4_kernel<true> : act_bwd_reduce_v4_kernel<false>), grid, 256,
+               0, G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, ws, M, C, p, slot);
     *rc = launch_status();
     if (*rc) return true;
     // the [chunk][2][C] partials are 2*chunks rows of C: even rows -> s1, odd rows -> s2
-    SPG_LAUNCH(K_ACT_BWD_REDUCE_FINAL, s, colsum_merge_kernel, (unsigned)ceil_div64(2 * C, 4), 128,
-               0, ws, chunks, 2 * C, s1 /* s1|s2 must be contiguous: see caller */);
+    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE_FINAL : K_ACT_BWD_REDUCE_FINAL, s, colsum_merge_kernel,
+               (unsigned)ceil_div64(2 * C, 4), 128, 0, ws, chunks, 2 * C, s12);
     *rc = launch_status();
-    (void)s2;
     return true;
 }
 
@@ -266,23 +300,29 @@ bool vec_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float
 bool vec_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
                        const float* scale, const float* shift, const float* mean,
                        const float* var, float eps, int relu, int has_bn, const float* s1,
-                       const float* s2, float* dY, int64_t lddy, int64_t M, int C,
-                       cudaStream_t s, int* rc) {
+                       const float* s2, float* dY, int64_t lddy, int64_t M, int C, float p,
+                       const int64_t* slot, cudaStream_t s, int* rc) {
     if ((C & 3) || !ld4(ldg) || !ld4(lddy) || !al16(G) || !al16(dY)) return false;
     if (Y && (!ld4(ldy) || !al16(Y))) return false;
-    dim3 grid((unsigned)ceil_div64(C, 128), row_grid(M));
-    SPG_LAUNCH(K_ACT_BWD_APPLY, s, act_bwd_apply_v4_kernel, grid, 256, 0, G, ldg, Y, ldy, scale,
-               shift, mean, var, eps, relu, has_bn, s1, s2, dY, lddy, M, C);
+    const bool drop = slot != nullptr;
+    dim3 grid((unsigned)ceil_div64(C, 128), row_grid(M, C, drop));
+    SPG_LAUNCH(drop ? K_DROPOUT_BWD_APPLY : K_ACT_BWD_APPLY, s,
+               (drop ? act_bwd_apply_v4_kernel<true> : act_bwd_apply_v4_kernel<false>), grid, 256,
+               0, G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, dY, lddy, M,
+               C, p, slot);
     *rc = launch_status();
     return true;
 }
 
 bool vec_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                    float* out, int64_t ldo, int64_t M, int C, cudaStream_t s, int* rc) {
+                    float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* slot,
+                    cudaStream_t s, int* rc) {
     if ((C & 3) || !ld4(ldy) || !ld4(ldo) || !al16(Y) || !al16(out)) return false;
-    dim3 grid((unsigned)ceil_div64(C, 128), row_grid(M));
-    SPG_LAUNCH(K_AFFINE_ACT, s, affine_act_v4_kernel, grid, 256, 0, Y, ldy, scale, shift, relu, out,
-               ldo, M, C);
+    const bool drop = slot != nullptr;
+    dim3 grid((unsigned)ceil_div64(C, 128), row_grid(M, C, drop));
+    SPG_LAUNCH(drop ? K_DROPOUT_FWD : K_AFFINE_ACT, s,
+               (drop ? affine_act_v4_kernel<true> : affine_act_v4_kernel<false>), grid, 256, 0, Y,
+               ldy, scale, shift, relu, out, ldo, M, C, p, slot);
     *rc = launch_status();
     return true;
 }

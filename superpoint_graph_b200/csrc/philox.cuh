@@ -50,11 +50,44 @@ __host__ __device__ __forceinline__ Philox4 dropout_words(uint64_t seed, uint64_
                          (uint32_t)(seed >> 32));
 }
 
-// Keep threshold: an element is kept iff its word >= floor(p * 2^32); p >= 1 drops everything (see drop_all).
+// Keep threshold: an element is kept iff its word >= floor(p * 2^32); p >= 1 drops everything (DropParams::all).
 __host__ __device__ __forceinline__ uint32_t dropout_threshold(float p) {
     if (!(p > 0.f)) return 0u;
     const double t = (double)p * 4294967296.0;
     return t >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)t;
+}
+
+// Per-launch dropout state, read from a slot (seed, ctr) in device memory.
+struct DropParams {
+    uint64_t seed, ctr;
+    uint32_t thr;
+    bool all;   // p >= 1: every element dropped
+    float inv;  // 1 / (1 - p)
+};
+
+__device__ __forceinline__ DropParams drop_params(const int64_t* slot, float p) {
+    DropParams d;
+    d.seed = (uint64_t)slot[0];
+    d.ctr = (uint64_t)slot[1];
+    d.thr = dropout_threshold(p);
+    d.all = !(p < 1.f);
+    d.inv = d.all ? 0.f : 1.f / (1.f - p);
+    return d;
+}
+
+__device__ __forceinline__ bool kept(const DropParams& d, uint32_t w) { return !d.all && w >= d.thr; }
+
+__device__ __forceinline__ uint32_t word_of(const Philox4& w, int64_t i) {
+    const int k = (int)(i & 3);
+    return k == 0 ? w.v[0] : k == 1 ? w.v[1] : k == 2 ? w.v[2] : w.v[3];
+}
+
+// G * m / (1-p) for one element (a select, so that p = 1 or an infinite gradient gives 0, never NaN)
+__device__ __forceinline__ float drop1(const DropParams& d, uint32_t w, float g) { return kept(d, w) ? g * d.inv : 0.f; }
+
+// drop1 of the element with logical index i, one Philox call for this element alone
+__device__ __forceinline__ float drop_at(const DropParams& d, int64_t i, float g) {
+    return drop1(d, word_of(dropout_words(d.seed, d.ctr, (uint64_t)(i >> 2)), i), g);
 }
 
 }  // namespace spg

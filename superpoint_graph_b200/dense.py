@@ -180,7 +180,7 @@ def chain_forward(inp, M, specs, params, training, saved=None):
             # dropout cannot ride in a GEMM prologue: BatchNorm-apply, ReLU and the mask in one pass, and
             # the consumer (next layer's GEMM and weight gradient) reads the dropped activation as is
             nxt.drop = (sp.drop, ops.dropout_slot(y.device))
-            act = Deferred(ops.dropout_fwd(y, sp.cout, M, sp.cout, scale, shift, sp.relu, sp.drop, nxt.drop[1]),
+            act = Deferred(ops.affine_act(y, sp.cout, M, sp.cout, scale, shift, sp.relu, drop=nxt.drop),
                            sp.cout, sp.cout)
         if saved is not None:
             saved.append((cur, nxt, mean, var))
@@ -205,9 +205,9 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
     act_bwd_reduce / act_bwd_apply kernels remain for the small-row chains.
 
     A layer with dropout masks the incoming gradient inside its own BatchNorm/ReLU backward
-    (dropout_bwd_reduce / dropout_bwd_apply, the mask regenerated from the forward's slot); both fused
-    paths that would read that gradient unmasked are off for it: the lazy prologue of its data-gradient
-    GEMM and the epilogue sums of the GEMM of the layer above."""
+    (act_bwd_reduce / act_bwd_apply with `drop`, the mask regenerated from the forward's slot); both
+    fused paths that would read that gradient unmasked are off for it: the lazy prologue of its
+    data-gradient GEMM and the epilogue sums of the GEMM of the layer above."""
     red = None  # s1|s2 of the current layer, if the GEMM that produced G already reduced them
     for li in range(len(specs) - 1, -1, -1):
         sp = specs[li]
@@ -233,13 +233,9 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
                 grads[sp.beta] = s1
         elif sp.bn is not None:
             eps = sp.bn.eps
-            if drop is not None:
-                assert red is None  # the layer above never reduces for a dropout layer (see bnred)
-                s12 = ops.dropout_bwd_reduce(G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps,
-                                             nxt.relu, drop[0], drop[1], M, C)
-            else:
-                s12 = red if red is not None else ops.act_bwd_reduce(
-                    G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps, nxt.relu, M, C)
+            assert drop is None or red is None  # the layer above never reduces for a dropout layer (see bnred)
+            s12 = red if red is not None else ops.act_bwd_reduce(
+                G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps, nxt.relu, M, C, drop=drop)
             s1, s2 = s12[:C], s12[C:]
             if sp.gamma is not None:
                 grads[sp.gamma] = s2
@@ -247,23 +243,14 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
             if (ops.USE_FUSED_BNBWD[0] and want_dx and ldg % 4 == 0 and nxt.ld % 4 == 0 and mean is not None
                     and drop is None and ops.tc_supported(M, sp.cin, sp.cout, ldg, sp.cin)):
                 lazy = (nxt.raw, nxt.ld, nxt.scale, nxt.shift, nxt.relu, mean, var, s12, eps, True)
-            elif drop is not None:
-                out = G if (own_g and ldg == C) else None
-                dY = ops.dropout_bwd_apply(G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps,
-                                           nxt.relu, True, s1, s2, drop[0], drop[1], M, C, out=out, ldo=C)
             else:
                 out = G if (own_g and ldg == C) else None
                 dY = ops.act_bwd_apply(G, ldg, nxt.raw, nxt.ld, nxt.scale, nxt.shift, mean, var, eps,
-                                       nxt.relu, True, s1, s2, M, C, out=out, ldo=C)
-        elif drop is not None:
+                                       nxt.relu, True, s1, s2, M, C, out=out, ldo=C, drop=drop)
+        elif sp.relu or drop is not None:
             out = G if (own_g and ldg == C) else None
-            dY = ops.dropout_bwd_apply(G, ldg, nxt.raw if sp.relu else None, nxt.ld, nxt.scale, nxt.shift, None,
-                                       None, 0.0, sp.relu, False, None, None, drop[0], drop[1], M, C,
-                                       out=out, ldo=C)
-        elif sp.relu:
-            out = G if (own_g and ldg == C) else None
-            dY = ops.act_bwd_apply(G, ldg, nxt.raw, nxt.ld, None, None, None, None, 0.0, True,
-                                   False, None, None, M, C, out=out, ldo=C)
+            dY = ops.act_bwd_apply(G, ldg, nxt.raw if sp.relu else None, nxt.ld, None, None, None, None, 0.0,
+                                   sp.relu, False, None, None, M, C, out=out, ldo=C, drop=drop)
         else:
             dY, ldy = G, ldg
         red = None

@@ -530,12 +530,21 @@ def bn_fold(mean, var, gamma, beta, eps, running_mean=None, running_var=None, mo
     return scale, shift
 
 
-def affine_act(Y, ldy, M, C, scale=None, shift=None, relu=False, out=None, ldo=None):
+def _drop(drop):
+    """drop = (p, slot) of a training-mode dropout, or None -> the (p, drop_slot) arguments of the C-ABI."""
+    if drop is None:
+        return 0.0, None
+    _need_cuda(drop[1])
+    return float(drop[0]), drop[1]
+
+
+def affine_act(Y, ldy, M, C, scale=None, shift=None, relu=False, out=None, ldo=None, drop=None):
+    """relu?(Y*scale+shift) -> [M, C]; with drop = (p, slot), dropout of that, mask from `slot`."""
     _need_cuda(Y)
     if out is None:
         out = torch.empty((M, C), dtype=torch.float32, device=Y.device)
         ldo = C
-    _lib.call("spg_affine_act", Y, ldy, scale, shift, int(bool(relu)), out, ldo, M, C,
+    _lib.call("spg_affine_act", Y, ldy, scale, shift, int(bool(relu)), out, ldo, M, C, *_drop(drop),
               _lib.current_stream())
     return out
 
@@ -548,25 +557,27 @@ def colsum(X, ldx, M, C):
     return out
 
 
-def act_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, M, C):
+def act_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, M, C, drop=None):
+    """-> s12 [2C]: s1 = s12[:C] (sum of the masked gradient), s2 = s12[C:] (same, weighted by xhat).
+    With drop = (p, slot), the gradient is first turned into G*m/(1-p), m regenerated from `slot`."""
     _need_cuda(G, Y)
-    """-> s12 [2C]: s1 = s12[:C] (sum of the masked gradient), s2 = s12[C:] (same, weighted by xhat)."""
     s12 = torch.empty(2 * C, dtype=torch.float32, device=G.device)
-    s1, s2 = s12[:C], s12[C:]  # contiguous pair: one merge launch writes both
     ws = workspace(2 * C * _chunks(M), G.device)
     _lib.call("spg_act_bwd_reduce", G, ldg, Y, ldy, scale, shift, mean, var, float(eps),
-              int(bool(relu)), s1, s2, ws, M, C, _lib.current_stream())
+              int(bool(relu)), s12, ws, M, C, *_drop(drop), _lib.current_stream())
     return s12
 
 
 def act_bwd_apply(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, M, C,
-                  out=None, ldo=None):
+                  out=None, ldo=None, drop=None):
+    """BatchNorm/ReLU backward -> dY [M, C]; drop as in act_bwd_reduce."""
     _need_cuda(G)
     if out is None:
         out = torch.empty((M, C), dtype=torch.float32, device=G.device)
         ldo = C
     _lib.call("spg_act_bwd_apply", G, ldg, Y, ldy, scale, shift, mean, var, float(eps),
-              int(bool(relu)), int(bool(has_bn)), s1, s2, out, ldo, M, C, _lib.current_stream())
+              int(bool(relu)), int(bool(has_bn)), s1, s2, out, ldo, M, C, *_drop(drop),
+              _lib.current_stream())
     return out
 
 
@@ -622,12 +633,8 @@ def dropout_slot(device):
 
 
 def dropout_fwd(Y, ldy, M, C, scale, shift, relu, p, slot):
-    """dropout(relu?(Y*scale+shift)) -> [M, C], mask from `slot`."""
-    _need_cuda(Y, slot)
-    out = torch.empty((M, C), dtype=torch.float32, device=Y.device)
-    _lib.call("spg_dropout_fwd", Y, ldy, scale, shift, int(bool(relu)), float(p), slot, out, C, M, C,
-              _lib.current_stream())
-    return out
+    """dropout(relu?(Y*scale+shift)) -> [M, C], mask from `slot` (affine_act with drop=(p, slot))."""
+    return affine_act(Y, ldy, M, C, scale, shift, relu, drop=(p, slot))
 
 
 def dropout_mask(slot, p, M, C):
@@ -636,28 +643,6 @@ def dropout_mask(slot, p, M, C):
     mask = torch.empty((M, C), dtype=torch.uint8, device=slot.device)
     _lib.call("spg_dropout_mask", _c(slot), float(p), M, C, mask, _lib.current_stream())
     return mask
-
-
-def dropout_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, p, slot, M, C):
-    """act_bwd_reduce of the gradient G*m/(1-p) -> s12 [2C]."""
-    _need_cuda(G, Y, slot)
-    s12 = torch.empty(2 * C, dtype=torch.float32, device=G.device)
-    ws = workspace(2 * C * _chunks(M), G.device)
-    _lib.call("spg_dropout_bwd_reduce", G, ldg, Y, ldy, scale, shift, mean, var, float(eps), int(bool(relu)),
-              float(p), slot, s12, ws, M, C, _lib.current_stream())
-    return s12
-
-
-def dropout_bwd_apply(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, p, slot, M, C,
-                      out=None, ldo=None):
-    """act_bwd_apply of the gradient G*m/(1-p) -> dY [M, C]."""
-    _need_cuda(G, slot)
-    if out is None:
-        out = torch.empty((M, C), dtype=torch.float32, device=G.device)
-        ldo = C
-    _lib.call("spg_dropout_bwd_apply", G, ldg, Y, ldy, scale, shift, mean, var, float(eps), int(bool(relu)),
-              int(bool(has_bn)), s1, s2, float(p), slot, out, ldo, M, C, _lib.current_stream())
-    return out
 
 
 # ------------------------------------------------------------------------- PointNet
