@@ -102,6 +102,8 @@ bool vec_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
 bool vec_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
                     float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* slot,
                     cudaStream_t s, int* rc);
+// out[c] = sum_k ws[k*C + c] for k < chunks (fp64, fixed order; dense_vec.cu), counted as kernel `kid`.
+int colsum_merge(int kid, const float* ws, int64_t chunks, int C, float* out, cudaStream_t s);
 
 }  // namespace spg
 

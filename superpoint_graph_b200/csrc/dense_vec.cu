@@ -248,6 +248,11 @@ affine_act_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __re
     }
 }
 
+int colsum_merge(int kid, const float* ws, int64_t chunks, int C, float* out, cudaStream_t s) {
+    SPG_LAUNCH(kid, s, colsum_merge_kernel, (unsigned)ceil_div64(C, 4), 128, 0, ws, chunks, C, out);
+    return launch_status();
+}
+
 static inline bool al16(const void* p) { return ((uintptr_t)p & 15) == 0; }
 static inline bool ld4(int64_t ld) { return (ld & 3) == 0; }
 
@@ -276,9 +281,7 @@ bool vec_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy
     *rc = launch_status();
     if (*rc) return true;
     // the [chunk][2][C] partials are 2*chunks rows of C: even rows -> s1, odd rows -> s2
-    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE_FINAL : K_ACT_BWD_REDUCE_FINAL, s, colsum_merge_kernel,
-               (unsigned)ceil_div64(2 * C, 4), 128, 0, ws, chunks, 2 * C, s12);
-    *rc = launch_status();
+    *rc = colsum_merge(drop ? K_DROPOUT_BWD_REDUCE_FINAL : K_ACT_BWD_REDUCE_FINAL, ws, chunks, 2 * C, s12, s);
     return true;
 }
 
@@ -291,9 +294,7 @@ bool vec_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float
     SPG_LAUNCH(K_COLSUM_PARTIAL, s, colsum_v4_kernel, grid, 256, 0, X, ldx, M, C, ws);
     *rc = launch_status();
     if (*rc) return true;
-    SPG_LAUNCH(K_COLSUM_FINAL, s, colsum_merge_kernel, (unsigned)ceil_div64(C, 4), 128, 0, ws,
-               chunks, C, out);
-    *rc = launch_status();
+    *rc = colsum_merge(K_COLSUM_FINAL, ws, chunks, C, out, s);
     return true;
 }
 

@@ -4,8 +4,7 @@
 // CloudEmbedder.
 //
 // Reference semantics: learning/pointnet.py:120-133 (transform + max_pool1d + cat),
-// :147-158 (index_copy_ into zero descriptors).  Segment boundaries are implicit
-// (constant L per superpoint, as the reference's loader guarantees: spg.py:209-214).
+// :147-158 (index_copy_ into zero descriptors).
 #include <float.h>
 
 #include "common.cuh"
@@ -13,6 +12,29 @@
 namespace spg {
 
 constexpr int kPtChunk = 128;
+
+// Segment layouts of the point rows the max-pool reduces.  The pooling kernels are templated on them.
+// Fixed-length clouds (the reference's loader resamples every superpoint to L points,
+// spg.py:209-214): segment b is rows [b*L, (b+1)*L).
+struct FixedSegs {
+    static constexpr bool kMayBeEmpty = false;  // L > 0
+    int L;
+    __device__ int64_t begin(int64_t b) const { return b * L; }
+    __device__ int64_t end(int64_t b) const { return (b + 1) * L; }
+    __device__ int64_t seg_of(int64_t r) const { return r / L; }
+};
+
+// Ragged CSR segments (north_star: "ragged segment boundaries carried as a CSR offset array"), the
+// variant WITHOUT that resampling: segment b is rows [offsets[b], offsets[b+1]), row_seg[r] is the
+// segment of row r.  An empty segment pools to 0 with argmax -1.
+struct CsrSegs {
+    static constexpr bool kMayBeEmpty = true;
+    const int64_t* offsets;
+    const int32_t* row_seg;
+    __device__ int64_t begin(int64_t b) const { return offsets[b]; }
+    __device__ int64_t end(int64_t b) const { return offsets[b + 1]; }
+    __device__ int64_t seg_of(int64_t r) const { return row_seg[r]; }
+};
 
 // grid (B, ceil(L/128)); block 128.  smem tile [F][129].
 __global__ void __launch_bounds__(kPtChunk)
@@ -48,22 +70,28 @@ cloud_rows_kernel(const float* __restrict__ clouds, const float* __restrict__ T,
     }
 }
 
+// pooled[b, c] = max over the rows of segment b, argmax[b, c] = index of the first maximum within the
+// segment.  A warp owns (segment, 32 channels): lane = channel for coalesced 128-byte row reads, the
+// segment's rows are strided over the 8 warps of the block and folded through shared memory.
 // grid (ceil(C/32), B); block (32 x 8).
+template <class Segs>
 __global__ void __launch_bounds__(256)
 segmax_fwd_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
                   const float* __restrict__ shift, int relu, float* __restrict__ pooled,
-                  int64_t ldp, int* __restrict__ argmax, int L, int C) {
+                  int64_t ldp, int* __restrict__ argmax, Segs segs, int C) {
     SPG_PDL_ENTRY();
     __shared__ float s_v[8][32];
     __shared__ int s_i[8][32];
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = blockIdx.x * 32 + x;
     const int64_t b = blockIdx.y;
+    const int64_t r0 = segs.begin(b);
+    const int L = (int)(segs.end(b) - r0);
     float best = -FLT_MAX;
     int bi = 0;
     if (c < C) {
         const float sc = scale ? scale[c] : 1.f, sh = shift ? shift[c] : 0.f;
-        const float* src = Y + b * L * ldy + c;
+        const float* src = Y + r0 * ldy + c;
         for (int l = y; l < L; l += 8) {
             float v = fmaf(__ldg(src + (int64_t)l * ldy), sc, sh);
             if (relu) v = fmaxf(v, 0.f);
@@ -87,23 +115,26 @@ segmax_fwd_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restr
                 bidx = i;
             }
         }
-        pooled[b * ldp + c] = bv;
+        pooled[b * ldp + c] = (Segs::kMayBeEmpty && bidx < 0) ? 0.f : bv;
         argmax[b * C + c] = bidx;
     }
 }
 
 // 128-bit variant: a warp spans 128 columns (float4 per lane), 8 row lanes, 4 rows in flight per
 // thread.  grid (ceil(C/128), B); block 256.  Same tie rule as the scalar kernel (first maximum).
+template <class Segs>
 __global__ void __launch_bounds__(256)
 segmax_fwd_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
                      const float* __restrict__ shift, int relu, float* __restrict__ pooled,
-                     int64_t ldp, int* __restrict__ argmax, int L, int C) {
+                     int64_t ldp, int* __restrict__ argmax, Segs segs, int C) {
     SPG_PDL_ENTRY();
     __shared__ float4 s_v[8][32];
     __shared__ int4 s_i[8][32];
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = (blockIdx.x * 32 + x) * 4;
     const int64_t b = blockIdx.y;
+    const int64_t r0 = segs.begin(b);
+    const int L = (int)(segs.end(b) - r0);
     float best[4] = {-FLT_MAX, -FLT_MAX, -FLT_MAX, -FLT_MAX};
     int bi[4] = {-1, -1, -1, -1};
     if (c < C) {
@@ -113,7 +144,7 @@ segmax_fwd_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __re
             if (scale) sc[j] = scale[c + j];
             if (shift) sh[j] = shift[c + j];
         }
-        const float* src = Y + b * L * ldy + c;
+        const float* src = Y + r0 * ldy + c;
 #pragma unroll 4
         for (int l = y; l < L; l += 8) {
             const float4 q = __ldg(reinterpret_cast<const float4*>(src + (int64_t)l * ldy));
@@ -147,21 +178,23 @@ segmax_fwd_v4_kernel(const float* __restrict__ Y, int64_t ldy, const float* __re
             }
         }
 #pragma unroll
-        for (int k = 0; k < 4; ++k) pooled[b * ldp + c + k] = best[k];
+        for (int k = 0; k < 4; ++k) pooled[b * ldp + c + k] = (Segs::kMayBeEmpty && bi[k] < 0) ? 0.f : best[k];
         *reinterpret_cast<int4*>(argmax + b * C + c) = make_int4(bi[0], bi[1], bi[2], bi[3]);
     }
 }
 
+// G[r, c] = g_pooled[b, c] if row r is the argmax of its segment b, else 0 (every row written).
+template <class Segs>
 __global__ void __launch_bounds__(256)
 segmax_bwd_kernel(const float* __restrict__ gp, int64_t ldg, const int* __restrict__ argmax,
-                  float* __restrict__ G, int64_t ldG, int64_t rows, int L, int C) {
+                  float* __restrict__ G, int64_t ldG, int64_t rows, Segs segs, int C) {
     SPG_PDL_ENTRY();
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = blockIdx.x * 32 + x;
     if (c >= C) return;
     for (int64_t r = (int64_t)blockIdx.y * 8 + y; r < rows; r += (int64_t)gridDim.y * 8) {
-        const int64_t b = r / L;
-        const int l = (int)(r % L);
+        const int64_t b = segs.seg_of(r);
+        const int l = (int)(r - segs.begin(b));
         G[r * ldG + c] = (argmax[b * C + c] == l) ? gp[b * ldg + c] : 0.f;
     }
 }
@@ -204,12 +237,13 @@ stn_apply_bwd_kernel(const float* __restrict__ clouds, const float* __restrict__
 // The gradient w.r.t. the pooled activation is non-zero at one point per (cloud, channel) only, so
 // the batch reductions s1 = sum G*mask, s2 = sum G*mask*xhat need just the argmax rows ...
 // grid (ceil(C/32), ceil(B/256)); block 32 x 8; partial layout [chunk][2][C] (as act_bwd_reduce).
+template <class Segs>
 __global__ void __launch_bounds__(256)
 segmax_bn_bwd_reduce_kernel(const float* __restrict__ gp, int64_t ldg, const int* __restrict__ argmax,
                             const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
                             const float* __restrict__ shift, const float* __restrict__ mean,
                             const float* __restrict__ var, float eps, int relu,
-                            float* __restrict__ ws, int64_t B, int L, int C) {
+                            float* __restrict__ ws, int64_t B, Segs segs, int C) {
     SPG_PDL_ENTRY();
     __shared__ float s1[8][32], s2[8][32];
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
@@ -221,7 +255,8 @@ segmax_bn_bwd_reduce_kernel(const float* __restrict__ gp, int64_t ldg, const int
         const float rstd = 1.f / sqrtf(var[c] + eps);
         for (int64_t b = b0 + y; b < b1; b += 8) {
             const int l = argmax[b * C + c];
-            const float yv = __ldg(Y + (b * L + l) * ldy + c);
+            if (Segs::kMayBeEmpty && l < 0) continue;  // empty segment: no row, no gradient
+            const float yv = __ldg(Y + (segs.begin(b) + l) * ldy + c);
             float g = __ldg(gp + b * ldg + c);
             if (relu && !(fmaf(yv, sc, sh) > 0.f)) g = 0.f;
             a1 += g;
@@ -243,19 +278,19 @@ segmax_bn_bwd_reduce_kernel(const float* __restrict__ gp, int64_t ldg, const int
 }
 
 // ... and dY = scale*(G*mask - s1/M - xhat*s2/M) is written directly from (g_pooled, argmax, Y):
-// the dense G is never materialised.  One 128-bit lane per 4 channels; M = B*L rows.
+// the dense G is never materialised.  One 128-bit lane per 4 channels; M rows in all segments.
+template <class Segs>
 __global__ void __launch_bounds__(256)
 segmax_bn_bwd_apply_kernel(const float* __restrict__ gp, int64_t ldg, const int* __restrict__ argmax,
                            const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
                            const float* __restrict__ shift, const float* __restrict__ mean,
                            const float* __restrict__ var, float eps, int relu,
                            const float* __restrict__ s1, const float* __restrict__ s2,
-                           float* __restrict__ dY, int64_t lddy, int64_t B, int L, int C) {
+                           float* __restrict__ dY, int64_t lddy, int64_t M, Segs segs, int C) {
     SPG_PDL_ENTRY();
     const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
     const int c = (blockIdx.x * 32 + x) * 4;
     if (c >= C) return;
-    const int64_t M = B * L;
     float sc[4], sh[4], mu[4], rs[4], m1[4], m2[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -268,8 +303,8 @@ segmax_bn_bwd_apply_kernel(const float* __restrict__ gp, int64_t ldg, const int*
     }
 #pragma unroll 2
     for (int64_t r = (int64_t)blockIdx.y * 8 + y; r < M; r += (int64_t)gridDim.y * 8) {
-        const int64_t b = r / L;
-        const int l = (int)(r - b * L);
+        const int64_t b = segs.seg_of(r);
+        const int l = (int)(r - segs.begin(b));
         const float4 yq = __ldg(reinterpret_cast<const float4*>(Y + r * ldy + c));
         const int4 am = __ldg(reinterpret_cast<const int4*>(argmax + b * C + c));
         // the pooled gradient row may be unaligned (ld = 256 + #global features): scalar loads, L1 hits
@@ -286,20 +321,6 @@ segmax_bn_bwd_apply_kernel(const float* __restrict__ gp, int64_t ldg, const int*
         }
         *reinterpret_cast<float4*>(dY + r * lddy + c) = make_float4(d[0], d[1], d[2], d[3]);
     }
-}
-
-// out[c] = sum_k ws[k*C + c] in fp64, one warp per column (same as dense_vec.cu's merge).
-__global__ void __launch_bounds__(128)
-pool_colsum_merge_kernel(const float* __restrict__ ws, int64_t chunks, int C, float* __restrict__ out) {
-    SPG_PDL_ENTRY();
-    const int lane = threadIdx.x & 31;
-    const int c = blockIdx.x * 4 + (threadIdx.x >> 5);
-    if (c >= C) return;
-    double a = 0.0;
-    for (int64_t k = lane; k < chunks; k += 32) a += (double)__ldg(ws + k * C + c);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-    if (lane == 0) out[c] = (float)a;
 }
 
 __global__ void rows_scatter_kernel(const float* __restrict__ src, const int64_t* __restrict__ idx,
@@ -340,68 +361,7 @@ rows_to_clouds_kernel(const float* __restrict__ rows, int64_t ld, float* __restr
         for (int l = threadIdx.x; l < nl; l += kPtChunk) dst[(int64_t)f * L + l0 + l] = tile[f * (kPtChunk + 1) + l];
 }
 
-// ------------------------------------------------------------------ ragged (CSR) segments
-// north_star: "ragged segment boundaries carried as a CSR offset array and reduced by warp-shuffle
-// segmented max".  The reference never feeds ragged clouds (its loader resamples every superpoint to
-// ptn_npts points, spg.py:209-214); these kernels are the variant WITHOUT that resampling: point rows
-// [P, ld] of all superpoints back to back, offsets int64 [B+1].  A warp owns (segment, 32 channels):
-// lane = channel for coalesced 128-byte row reads, the segment's rows are strided over the 8 warps of
-// the block and folded through shared memory; ties keep the FIRST maximum (as max_pool1d).
-// argmax is the GLOBAL row index (int64), -1 for an empty segment (pooled value 0).
-__global__ void __launch_bounds__(256)
-segmax_csr_fwd_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
-                      const float* __restrict__ shift, int relu, const int64_t* __restrict__ offsets,
-                      float* __restrict__ pooled, int64_t ldp, int64_t* __restrict__ argmax, int C) {
-    SPG_PDL_ENTRY();
-    __shared__ float s_v[8][32];
-    __shared__ long long s_i[8][32];
-    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const int c = blockIdx.x * 32 + x;
-    const int64_t b = blockIdx.y;
-    const int64_t r0 = offsets[b], r1 = offsets[b + 1];
-    float best = -FLT_MAX;
-    long long bi = -1;
-    if (c < C) {
-        const float sc = scale ? scale[c] : 1.f, sh = shift ? shift[c] : 0.f;
-        for (int64_t r = r0 + y; r < r1; r += 8) {
-            float v = fmaf(__ldg(Y + r * ldy + c), sc, sh);
-            if (relu) v = fmaxf(v, 0.f);
-            if (bi < 0 || v > best) {
-                best = v;
-                bi = r;
-            }
-        }
-    }
-    s_v[y][x] = best;
-    s_i[y][x] = bi;
-    __syncthreads();
-    if (y == 0 && c < C) {
-        for (int j = 1; j < 8; ++j) {
-            const float v = s_v[j][x];
-            const long long i = s_i[j][x];
-            if (i >= 0 && (bi < 0 || v > best || (v == best && i < bi))) {
-                best = v;
-                bi = i;
-            }
-        }
-        pooled[b * ldp + c] = bi >= 0 ? best : 0.f;
-        argmax[b * C + c] = bi;
-    }
-}
-
-// G[P, C] = 0 except G[argmax[b,c], c] = g_pooled[b, c]   (G is zeroed by the launcher)
-__global__ void __launch_bounds__(256)
-segmax_csr_bwd_kernel(const float* __restrict__ gp, int64_t ldg, const int64_t* __restrict__ argmax,
-                      float* __restrict__ G, int64_t ldG, int64_t B, int C) {
-    SPG_PDL_ENTRY();
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B * C) return;
-    const int64_t b = i / C;
-    const int c = (int)(i % C);
-    const int64_t r = argmax[i];
-    if (r >= 0) G[r * ldG + c] = gp[b * ldg + c];
-}
-
+// ------------------------------------------------------------------ ragged (CSR) segments: the xy transform
 // rows_out = rows_in with columns 0,1 replaced by (x0,x1) * (T[seg] (+ I))   (pointnet.py:123)
 __global__ void __launch_bounds__(256)
 rows_xy_transform_kernel(const float* __restrict__ in, const float* __restrict__ T, int add_eye,
@@ -452,6 +412,12 @@ rows_xy_transform_bwd_kernel(const float* __restrict__ in, int64_t ld, const flo
     }
 }
 
+// f(segs) with the layout a C-ABI call describes: fixed length L if offsets is NULL, else CSR.
+template <class F>
+static int with_segs(int L, const int64_t* offsets, const int32_t* row_seg, F&& f) {
+    return offsets ? f(CsrSegs{offsets, row_seg}) : f(FixedSegs{L});
+}
+
 }  // namespace spg
 
 using namespace spg;
@@ -478,9 +444,9 @@ int spg_cloud_rows(const float* clouds, const float* T, int add_eye, float* rows
 }
 
 int spg_segmax_fwd(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                   float* pooled, int64_t ldp, int32_t* argmax, int64_t B, int L, int C,
-                   spg_stream_t stream) {
-    if (B < 0 || L <= 0 || C <= 0 || ldy < C || ldp < C) return SPG_E_BADARG;
+                   float* pooled, int64_t ldp, int32_t* argmax, int64_t B, int L, const int64_t* offsets,
+                   int C, spg_stream_t stream) {
+    if (B < 0 || (!offsets && L <= 0) || C <= 0 || ldy < C || ldp < C) return SPG_E_BADARG;
     if (B == 0) return SPG_OK;
     if (!Y || !pooled || !argmax) return SPG_E_BADARG;
     if (B > 65535ll * 32768) return SPG_E_UNSUPPORTED;
@@ -490,64 +456,71 @@ int spg_segmax_fwd(const float* Y, int64_t ldy, const float* scale, const float*
                      ((uintptr_t)argmax & 15) == 0;
     for (int64_t b0 = 0; b0 < B; b0 += max_by) {
         const int64_t nb = min(max_by, B - b0);
-        if (vec) {
-            dim3 grid((unsigned)ceil_div64(C, 128), (unsigned)nb);
-            SPG_LAUNCH(K_SEGMAX_FWD, s, segmax_fwd_v4_kernel, grid, 256, 0, Y + b0 * L * ldy, ldy,
-                       scale, shift, relu, pooled + b0 * ldp, ldp, argmax + b0 * C, L, C);
-            int rcv = launch_status();
-            if (rcv) return rcv;
-            continue;
-        }
-        dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)nb);
-        SPG_LAUNCH(K_SEGMAX_FWD, s, segmax_fwd_kernel, grid, 256, 0, Y + b0 * L * ldy, ldy, scale,
-                   shift, relu, pooled + b0 * ldp, ldp, argmax + b0 * C, L, C);
-        int rc = launch_status();
+        // segments [b0, b0 + nb): the fixed layout moves Y, the CSR layout moves offsets
+        const float* Yb = offsets ? Y : Y + b0 * L * ldy;
+        const int rc = with_segs(L, offsets ? offsets + b0 : nullptr, nullptr, [&](auto segs) {
+            if (vec) {
+                dim3 grid((unsigned)ceil_div64(C, 128), (unsigned)nb);
+                SPG_LAUNCH(K_SEGMAX_FWD, s, segmax_fwd_v4_kernel<decltype(segs)>, grid, 256, 0, Yb, ldy,
+                           scale, shift, relu, pooled + b0 * ldp, ldp, argmax + b0 * C, segs, C);
+            } else {
+                dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)nb);
+                SPG_LAUNCH(K_SEGMAX_FWD, s, segmax_fwd_kernel<decltype(segs)>, grid, 256, 0, Yb, ldy,
+                           scale, shift, relu, pooled + b0 * ldp, ldp, argmax + b0 * C, segs, C);
+            }
+            return launch_status();
+        });
         if (rc) return rc;
     }
     return SPG_OK;
 }
 
 int spg_segmax_bwd(const float* g_pooled, int64_t ldg, const int32_t* argmax, float* G,
-                   int64_t ldG, int64_t B, int L, int C, spg_stream_t stream) {
-    if (B < 0 || L <= 0 || C <= 0 || ldg < C || ldG < C) return SPG_E_BADARG;
-    if (B == 0) return SPG_OK;
+                   int64_t ldG, int64_t B, int L, const int64_t* offsets, const int32_t* row_seg,
+                   int64_t rows, int C, spg_stream_t stream) {
+    if (B < 0 || rows < 0 || C <= 0 || ldg < C || ldG < C) return SPG_E_BADARG;
+    if (offsets ? !row_seg : (L <= 0 || rows != B * L)) return SPG_E_BADARG;
+    if (rows == 0) return SPG_OK;
     if (!g_pooled || !argmax || !G) return SPG_E_BADARG;
-    const int64_t rows = B * L;
     int64_t gy = ceil_div64(rows, 64);
     if (gy > 8 * kNumSMs) gy = 8 * kNumSMs;
     dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)gy);
-    SPG_LAUNCH(K_SEGMAX_BWD, (cudaStream_t)stream, segmax_bwd_kernel, grid, 256, 0, g_pooled, ldg,
-               argmax, G, ldG, rows, L, C);
-    return launch_status();
+    return with_segs(L, offsets, row_seg, [&](auto segs) {
+        SPG_LAUNCH(K_SEGMAX_BWD, (cudaStream_t)stream, segmax_bwd_kernel<decltype(segs)>, grid, 256, 0,
+                   g_pooled, ldg, argmax, G, ldG, rows, segs, C);
+        return launch_status();
+    });
 }
 
 int spg_segmax_bn_bwd(const float* g_pooled, int64_t ldg, const int32_t* argmax, const float* Y,
                       int64_t ldy, const float* scale, const float* shift, const float* mean,
                       const float* var, float eps, int relu, float* s12, float* dY, int64_t lddy,
-                      float* workspace, int64_t B, int L, int C, spg_stream_t stream) {
-    if (B <= 0 || L <= 0 || C <= 0 || !g_pooled || !argmax || !Y || !scale || !shift || !mean || !var ||
+                      float* workspace, int64_t B, int L, const int64_t* offsets, const int32_t* row_seg,
+                      int64_t rows, int C, spg_stream_t stream) {
+    if (B <= 0 || rows <= 0 || C <= 0 || !g_pooled || !argmax || !Y || !scale || !shift || !mean || !var ||
         !s12 || !dY || !workspace)
         return SPG_E_BADARG;
+    if (offsets ? !row_seg : (L <= 0 || rows != B * L)) return SPG_E_BADARG;
     if ((C & 3) || (ldy & 3) || (lddy & 3)) return SPG_E_UNSUPPORTED;
     if (((uintptr_t)argmax | (uintptr_t)Y | (uintptr_t)dY) & 15) return SPG_E_ALIGN;
     cudaStream_t s = (cudaStream_t)stream;
     const int64_t chunks = ceil_div64(B, 256);
     if (chunks > 65535) return SPG_E_UNSUPPORTED;
-    dim3 g1((unsigned)ceil_div64(C, 32), (unsigned)chunks);
-    SPG_LAUNCH(K_SEGMAX_BWD, s, segmax_bn_bwd_reduce_kernel, g1, 256, 0, g_pooled, ldg, argmax, Y, ldy,
-               scale, shift, mean, var, eps, relu, workspace, B, L, C);
-    int rc = launch_status();
-    if (rc) return rc;
-    SPG_LAUNCH(K_SEGMAX_BWD, s, pool_colsum_merge_kernel, (unsigned)ceil_div64(2 * C, 4), 128, 0, workspace,
-               chunks, 2 * C, s12);
-    rc = launch_status();
-    if (rc) return rc;
-    int64_t gy = ceil_div64(B * L, 32);
-    if (gy > 16 * kNumSMs) gy = 16 * kNumSMs;
-    dim3 g2((unsigned)ceil_div64(C, 128), (unsigned)gy);
-    SPG_LAUNCH(K_SEGMAX_BWD, s, segmax_bn_bwd_apply_kernel, g2, 256, 0, g_pooled, ldg, argmax, Y, ldy, scale,
-               shift, mean, var, eps, relu, s12, s12 + C, dY, lddy, B, L, C);
-    return launch_status();
+    return with_segs(L, offsets, row_seg, [&](auto segs) {
+        dim3 g1((unsigned)ceil_div64(C, 32), (unsigned)chunks);
+        SPG_LAUNCH(K_SEGMAX_BWD, s, segmax_bn_bwd_reduce_kernel<decltype(segs)>, g1, 256, 0, g_pooled, ldg,
+                   argmax, Y, ldy, scale, shift, mean, var, eps, relu, workspace, B, segs, C);
+        int rc = launch_status();
+        if (rc) return rc;
+        rc = colsum_merge(K_SEGMAX_BWD, workspace, chunks, 2 * C, s12, s);
+        if (rc) return rc;
+        int64_t gy = ceil_div64(rows, 32);
+        if (gy > 16 * kNumSMs) gy = 16 * kNumSMs;
+        dim3 g2((unsigned)ceil_div64(C, 128), (unsigned)gy);
+        SPG_LAUNCH(K_SEGMAX_BWD, s, segmax_bn_bwd_apply_kernel<decltype(segs)>, g2, 256, 0, g_pooled, ldg,
+                   argmax, Y, ldy, scale, shift, mean, var, eps, relu, s12, s12 + C, dY, lddy, rows, segs, C);
+        return launch_status();
+    });
 }
 
 int spg_stn_apply_bwd(const float* clouds, const float* dXrows, int64_t ld, float* dT, int64_t B,
@@ -591,33 +564,6 @@ int spg_rows_to_clouds(const float* rows, int64_t ld, float* clouds, int64_t B, 
     dim3 grid((unsigned)B, (unsigned)ceil_div64(L, kPtChunk));
     SPG_LAUNCH(K_CLOUD_ROWS, (cudaStream_t)stream, rows_to_clouds_kernel, grid, kPtChunk, smem, rows, ld, clouds, F,
                L);
-    return launch_status();
-}
-
-int spg_segmax_csr_fwd(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                       const int64_t* offsets, float* pooled, int64_t ldp, int64_t* argmax_row, int64_t B,
-                       int C, spg_stream_t stream) {
-    if (B < 0 || C <= 0 || ldy < C || ldp < C) return SPG_E_BADARG;
-    if (B == 0) return SPG_OK;
-    if (!Y || !offsets || !pooled || !argmax_row) return SPG_E_BADARG;
-    if (B > 65535) return SPG_E_UNSUPPORTED;  // grid.y
-    dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)B);
-    SPG_LAUNCH(K_SEGMAX_FWD, (cudaStream_t)stream, segmax_csr_fwd_kernel, grid, 256, 0, Y, ldy, scale, shift,
-               relu, offsets, pooled, ldp, (int64_t*)argmax_row, C);
-    return launch_status();
-}
-
-int spg_segmax_csr_bwd(const float* g_pooled, int64_t ldg, const int64_t* argmax_row, float* G, int64_t ldG,
-                       int64_t B, int C, int64_t P, spg_stream_t stream) {
-    if (B < 0 || C <= 0 || P < 0 || ldG < C || ldg < C) return SPG_E_BADARG;
-    if (P == 0) return SPG_OK;
-    if (!G) return SPG_E_BADARG;
-    cudaError_t e = cudaMemsetAsync(G, 0, (size_t)P * ldG * sizeof(float), (cudaStream_t)stream);
-    if (e != cudaSuccess) return (int)e;
-    if (B == 0) return SPG_OK;
-    if (!g_pooled || !argmax_row) return SPG_E_BADARG;
-    SPG_LAUNCH(K_SEGMAX_BWD, (cudaStream_t)stream, segmax_csr_bwd_kernel, (unsigned)ceil_div64(B * C, 256), 256,
-               0, g_pooled, ldg, argmax_row, G, ldG, B, C);
     return launch_status();
 }
 

@@ -196,7 +196,8 @@ def _accumulate_grad(prm, g):
 def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_g=False, pooled=None):
     """G: gradient w.r.t. the chain's final *activated* output [M, C_last].
     `grads` (list aligned with params) is filled in place.  Returns the gradient w.r.t. the
-    chain input's activated value [M, cin_0] (or None).
+    chain input's activated value [M, cin_0] (or None).  If the chain's output was max-pooled over the
+    segments `seg` (ops.segmax_fwd), G is None and pooled = (g_pooled, ldg, argmax, seg).
 
     Where the data-gradient GEMM of a layer runs on the wgmma kernel, the BatchNorm/ReLU backward
     around it is fused into that ONE launch: the prologue turns dL/d(activation) into dL/dY on the
@@ -219,15 +220,15 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
         fused_pool = (pooled is not None and li == len(specs) - 1 and sp.bn is not None
                       and mean is not None and C % 4 == 0 and drop is None)
         if G is None and not fused_pool:  # generic path: materialise the dense pooled gradient
-            gp, ldgp, argmax, Bc, Lc = pooled
-            G, ldg, own_g = ops.segmax_bwd(gp, ldgp, argmax, Bc, Lc, C), C, True
+            gp, ldgp, argmax, seg = pooled
+            G, ldg, own_g = ops.segmax_bwd(gp, ldgp, argmax, seg, C), C, True
         lazy = None  # BatchNorm backward deferred into the data-gradient GEMM's prologue
         dY, ldy = None, C
         if fused_pool:
             # the chain's output went through a max-pool: fused pool-backward + BN/ReLU backward
-            gp, ldgp, argmax, Bc, Lc = pooled
+            gp, ldgp, argmax, seg = pooled
             s1, s2, dY = ops.segmax_bn_bwd(gp, ldgp, argmax, nxt.raw, nxt.ld, nxt.scale, nxt.shift,
-                                           mean, var, sp.bn.eps, nxt.relu, Bc, Lc, C)
+                                           mean, var, sp.bn.eps, nxt.relu, seg, C)
             if sp.gamma is not None:
                 grads[sp.gamma] = s2
                 grads[sp.beta] = s1

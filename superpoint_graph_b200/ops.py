@@ -663,30 +663,49 @@ def rows_to_clouds(rows, ld, B, F, L):
     return out
 
 
-def segmax_fwd(Y, ldy, B, L, C, scale, shift, relu, pooled, ldp):
-    _need_cuda(Y, pooled)
+def _seg_rows(seg):
+    """Row count of a segment description seg = (B, L, offsets, row_seg): B segments of L rows if offsets
+    is None, else CSR segments [offsets[b], offsets[b+1]) (int64 [B+1]) with row_seg the int32 segment of
+    every row."""
+    B, L, offsets, row_seg = seg
+    if offsets is None:
+        return B * L
+    assert offsets.dtype == torch.int64 and offsets.is_contiguous() and row_seg.dtype == torch.int32
+    return row_seg.numel()
+
+
+def segmax_fwd(Y, ldy, seg, C, scale, shift, relu, pooled, ldp):
+    """Max-pool of relu?(Y*scale+shift) over each segment of seg into pooled[:, :C]; returns the int32
+    argmax within the segment (-1 for an empty segment, whose pooled value is 0)."""
+    B, L, offsets, _ = seg
+    _need_cuda(Y, pooled, offsets)
+    assert offsets is None or (offsets.dtype == torch.int64 and offsets.is_contiguous())
     argmax = torch.empty((B, C), dtype=torch.int32, device=Y.device)
-    _lib.call("spg_segmax_fwd", Y, ldy, scale, shift, int(bool(relu)), pooled, ldp, argmax, B, L, C,
+    _lib.call("spg_segmax_fwd", Y, ldy, scale, shift, int(bool(relu)), pooled, ldp, argmax, B, L, offsets, C,
               _lib.current_stream())
     return argmax
 
 
-def segmax_bwd(g_pooled, ldg, argmax, B, L, C):
+def segmax_bwd(g_pooled, ldg, argmax, seg, C):
     _need_cuda(g_pooled, argmax)
-    G = torch.empty((B * L, C), dtype=torch.float32, device=g_pooled.device)
-    _lib.call("spg_segmax_bwd", g_pooled, ldg, argmax, G, C, B, L, C, _lib.current_stream())
+    B, L, offsets, row_seg = seg
+    M = _seg_rows(seg)
+    G = torch.empty((M, C), dtype=torch.float32, device=g_pooled.device)
+    _lib.call("spg_segmax_bwd", g_pooled, ldg, argmax, G, C, B, L, offsets, row_seg, M, C, _lib.current_stream())
     return G
 
 
-def segmax_bn_bwd(g_pooled, ldg, argmax, Y, ldy, scale, shift, mean, var, eps, relu, B, L, C):
-    """Fused max-pool backward + BatchNorm/ReLU backward; returns (s1, s2, dY[B*L, C])."""
+def segmax_bn_bwd(g_pooled, ldg, argmax, Y, ldy, scale, shift, mean, var, eps, relu, seg, C):
+    """Fused max-pool backward + BatchNorm/ReLU backward; returns (s1, s2, dY[rows, C])."""
     _need_cuda(g_pooled, argmax, Y)
     dev = Y.device
+    B, L, offsets, row_seg = seg
+    M = _seg_rows(seg)
     s12 = torch.empty(2 * C, dtype=torch.float32, device=dev)
-    dY = torch.empty((B * L, C), dtype=torch.float32, device=dev)
+    dY = torch.empty((M, C), dtype=torch.float32, device=dev)
     ws = workspace(2 * C * ((B + 255) // 256), dev)
     _lib.call("spg_segmax_bn_bwd", g_pooled, ldg, argmax, Y, ldy, scale, shift, mean, var, float(eps),
-              int(bool(relu)), s12, dY, C, ws, B, L, C, _lib.current_stream())
+              int(bool(relu)), s12, dY, C, ws, B, L, offsets, row_seg, M, C, _lib.current_stream())
     return s12[:C], s12[C:], dY
 
 
@@ -906,23 +925,6 @@ def nn1_interpolate(xyz_ref, xyz_query, labels_ref=None, want_index=False):
 
 
 # ------------------------------------------------------------------ ragged (CSR) superpoints
-def segmax_csr_fwd(Y, ldy, offsets, C, scale, shift, relu, pooled, ldp):
-    _need_cuda(Y, offsets, pooled)
-    assert offsets.dtype == torch.int64 and offsets.is_contiguous()
-    B = offsets.numel() - 1
-    argmax = torch.empty((B, C), dtype=torch.int64, device=Y.device)
-    _lib.call("spg_segmax_csr_fwd", Y, ldy, scale, shift, int(bool(relu)), offsets, pooled, ldp, argmax, B, C,
-              _lib.current_stream())
-    return argmax
-
-
-def segmax_csr_bwd(g_pooled, ldg, argmax, P, C):
-    _need_cuda(g_pooled, argmax)
-    G = torch.empty((P, C), dtype=torch.float32, device=g_pooled.device)
-    _lib.call("spg_segmax_csr_bwd", g_pooled, ldg, argmax, G, C, argmax.shape[0], C, P, _lib.current_stream())
-    return G
-
-
 def rows_xy_transform(rows, T, row_seg, add_eye=True):
     _need_cuda(rows, T, row_seg)
     assert rows.is_contiguous() and row_seg.dtype == torch.int32

@@ -82,8 +82,23 @@ def _stn_groups(stn, training, params):
 
 
 # Segment layouts: everything of the PointNet forward/backward that depends on how the points of a
-# cloud are laid out.  Point rows are [M, ld] (one point per row, features zero-padded to ld).
-class _Clouds(object):
+# cloud are laid out.  Point rows are [M, ld] (one point per row, features zero-padded to ld); `seg` =
+# (B, L, offsets, row_seg) describes the segments to the pooling kernels (ops.segmax_fwd).
+class _Layout(object):
+    def segmax(self, out, pooled):
+        """Max over each segment of the Deferred point rows `out` into pooled[:, :out.C]; returns argmax."""
+        return ops.segmax_fwd(out.raw, out.ld, self.seg, out.C, out.scale, out.shift, out.relu, pooled,
+                              pooled.shape[1])
+
+    def segmax_backward(self, g_pool, specs, params, record, need_input_grad, grads):
+        """Backward of segmax and of the point-wise chain `specs` before it; returns the point-row gradient."""
+        saved, argmax = record
+        # chain_backward fuses the pool backward into the last layer's BatchNorm backward
+        return chain_backward(None, specs[-1].cout, self.M, specs, params, saved, need_input_grad, grads,
+                              pooled=(g_pool, g_pool.shape[1], argmax, self.seg))
+
+
+class _Clouds(_Layout):
     """Fixed-length clouds [B, F, L] (the reference's layout); point row b*L + l is point l of cloud b."""
 
     has_input_grad = True
@@ -94,22 +109,11 @@ class _Clouds(object):
         self.B, self.F, self.L = self.clouds.shape
         self.M = self.B * self.L
         self.ld = _row_ld(self.F)
+        self.seg = (self.B, self.L, None, None)
 
     def rows(self, T=None):
         """The point rows; with T [B, 4] the xy columns are transformed by T + I."""
         return ops.cloud_rows(self.clouds, T, self.ld, add_eye=T is not None)
-
-    def segmax(self, out, pooled):
-        """Max over each cloud's points of the Deferred point rows `out` into pooled[:, :out.C]; returns argmax."""
-        return ops.segmax_fwd(out.raw, out.ld, self.B, self.L, out.C, out.scale, out.shift, out.relu, pooled,
-                              pooled.shape[1])
-
-    def segmax_backward(self, g_pool, specs, params, record, need_input_grad, grads):
-        """Backward of segmax and of the point-wise chain `specs` before it; returns the point-row gradient."""
-        saved, argmax = record
-        # chain_backward fuses the pool backward into the last layer's BatchNorm backward
-        return chain_backward(None, specs[-1].cout, self.M, specs, params, saved, need_input_grad, grads,
-                              pooled=(g_pool, g_pool.shape[1], argmax, self.B, self.L))
 
     def xy_transform_backward(self, g_rows):
         """dT [B, 4] from the gradient w.r.t. the transformed point rows."""
@@ -135,7 +139,7 @@ class _Clouds(object):
         ops.pointnet_fused_eval(self.clouds, T, img, bias, widths, pooled, pooled.shape[1])
 
 
-class _Segments(object):
+class _Segments(_Layout):
     """Ragged superpoints as CSR segments: `points` [P, F] of all B superpoints back to back, int64
     `offsets` [B+1]; point row p is points[p]."""
 
@@ -153,21 +157,12 @@ class _Segments(object):
         # segment of every point row; built before any chain is queued, as it waits for the device
         self.row_seg = torch.repeat_interleave(torch.arange(self.B, device=self.device, dtype=torch.int32),
                                                self.offsets[1:] - self.offsets[:-1])
+        self.seg = (self.B, 0, self.offsets, self.row_seg)
 
     def rows(self, T=None):
         if T is None:
             return self.rows0
         return ops.rows_xy_transform(self.rows0, T, self.row_seg, add_eye=True)
-
-    def segmax(self, out, pooled):
-        return ops.segmax_csr_fwd(out.raw, out.ld, self.offsets, out.C, out.scale, out.shift, out.relu, pooled,
-                                  pooled.shape[1])
-
-    def segmax_backward(self, g_pool, specs, params, record, need_input_grad, grads):
-        saved, argmax = record
-        C = specs[-1].cout
-        G = ops.segmax_csr_bwd(g_pool, g_pool.shape[1], argmax, self.M, C)
-        return chain_backward(G, C, self.M, specs, params, saved, need_input_grad, grads, own_g=True)
 
     def xy_transform_backward(self, g_rows):
         return ops.rows_xy_transform_bwd(self.rows0, g_rows, self.offsets)

@@ -272,12 +272,25 @@ def test_batch_stats_and_bn_backward(dev, M, C):
     close(dY, Yr.grad, 1e-4, 1e-6)
 
 
-@pytest.mark.parametrize("L,C", [(128, 70), (128, 64), (128, 256), (20, 132), (7, 8)])
-def test_segmax_and_cloud_rows(dev, L, C):
-    """C = 70: scalar pooling kernel; C % 4 == 0: the 128-bit one (incl. L < 8 row lanes)."""
+def csr_seg(lens, dev):
+    """Segment description (B, L, offsets, row_seg) of CSR segments of the given lengths."""
+    lens = torch.as_tensor(lens, dtype=torch.int64)
+    offsets = torch.cat([torch.zeros(1, dtype=torch.int64), lens.cumsum(0)])
+    row_seg = torch.repeat_interleave(torch.arange(len(lens), dtype=torch.int32), lens)
+    return len(lens), 0, offsets.to(dev), row_seg.to(dev)
+
+
+@pytest.mark.parametrize("L,C,layout", [
+    pytest.param(L, C, layout, id="%d-%d%s" % (L, C, "-csr" if layout == "csr" else ""))
+    for layout in ("fixed", "csr") for L, C in [(128, 70), (128, 64), (128, 256), (20, 132), (7, 8)]])
+def test_segmax_and_cloud_rows(dev, L, C, layout):
+    """C = 70: scalar pooling kernel; C % 4 == 0: the 128-bit one (incl. L < 8 row lanes).  layout "csr":
+    the same equal-length segments given as CSR offsets, bit-identical to the fixed layout."""
     from superpoint_graph_b200 import ops
     torch.manual_seed(5)
     B, F = 37, 14
+    fixed = (B, L, None, None)
+    seg = fixed if layout == "fixed" else csr_seg([L] * B, dev)
     clouds = torch.randn(B, F, L, device=dev)
     T = torch.randn(B, 2, 2, device=dev)
     rows = ops.cloud_rows(clouds, T.reshape(B, 4), 16, add_eye=True)
@@ -289,27 +302,120 @@ def test_segmax_and_cloud_rows(dev, L, C):
     Y = torch.randn(B * L, C, device=dev)
     sc, sh = torch.randn(C, device=dev), torch.randn(C, device=dev)
     pooled = torch.empty(B, C + 2, device=dev)
-    am = ops.segmax_fwd(Y, C, B, L, C, sc, sh, True, pooled, C + 2)
+    am = ops.segmax_fwd(Y, C, seg, C, sc, sh, True, pooled, C + 2)
     a = torch.relu(Y * sc + sh).view(B, L, C)
     mx, idx = a.max(1)
     close(pooled[:, :C], mx, 1e-6)
     close(a.gather(1, am.long().unsqueeze(1)).squeeze(1), mx, 1e-6)  # argmax attains the max
+    if layout == "csr":
+        pooled_f = torch.empty(B, C + 2, device=dev)
+        assert torch.equal(am, ops.segmax_fwd(Y, C, fixed, C, sc, sh, True, pooled_f, C + 2))
+        assert torch.equal(pooled[:, :C], pooled_f[:, :C])
     # without the affine the arithmetic is exact: index output must be bit-exact, first maximiser
     Yq = torch.round(Y * 4) / 4  # many ties
-    am = ops.segmax_fwd(Yq, C, B, L, C, None, None, False, pooled, C + 2)
+    am = ops.segmax_fwd(Yq, C, seg, C, None, None, False, pooled, C + 2)
     a = Yq.view(B, L, C)
     mx, _ = a.max(1)
     assert torch.equal(pooled[:, :C], mx)
     first = (a == mx.unsqueeze(1)).float().argmax(1)
     assert torch.equal(am.long(), first)
     gp = torch.randn(B, C, device=dev)
-    G = ops.segmax_bwd(gp, C, am, B, L, C)
+    G = ops.segmax_bwd(gp, C, am, seg, C)
     ref = torch.zeros(B, L, C, device=dev).scatter_(1, am.long().unsqueeze(1), gp.unsqueeze(1))
     assert torch.equal(G.view(B, L, C), ref)
+    if layout == "csr":
+        assert torch.equal(G, ops.segmax_bwd(gp, C, am, fixed, C))
     dX = torch.randn(B * L, 16, device=dev)
     dT = ops.stn_apply_bwd(clouds, dX, 16)
     ref = torch.bmm(clouds[:, :2], dX.view(B, L, 16)[:, :, :2])
     close(dT.view(B, 2, 2), ref, 1e-5)
+
+
+def check_pool_vs_torch(ops, Y, seg, C, dev):
+    """segmax_fwd / segmax_bwd over the CSR segments `seg` of Y [P, C] against torch: the exact max (0 for
+    an empty segment), the FIRST maximiser within the segment (-1 for an empty one), the scattered gradient."""
+    B, _, offsets, row_seg = seg
+    P = Y.shape[0]
+    pooled = torch.empty(B, C, device=dev)
+    am = ops.segmax_fwd(Y, C, seg, C, None, None, False, pooled, C)
+    rs = row_seg.long()
+    lens = offsets[1:] - offsets[:-1]
+    mx = torch.full((B, C), -float("inf"), device=dev).scatter_reduce_(0, rs[:, None].expand(P, C), Y, "amax")
+    mx[lens == 0] = 0
+    assert torch.equal(pooled, mx)
+    assert torch.equal(am[lens == 0], torch.full_like(am[lens == 0], -1))
+    full = lens > 0
+    assert bool((am[full] >= 0).all()) and bool((am[full] < lens[full, None]).all())
+    rows = offsets[:-1, None] + am.long()
+    assert torch.equal(Y.gather(0, rows[full]), mx[full])  # the argmax attains the max ...
+    l_of_row = torch.arange(P, device=dev) - offsets[rs]
+    at_max = Y == mx[rs]
+    assert bool((l_of_row[:, None] >= am[rs])[at_max].all())  # ... and no earlier row of its segment does
+    gp = torch.randn(B, C, device=dev)
+    G = ops.segmax_bwd(gp, C, am, seg, C)
+    ref = torch.zeros(P, C, device=dev).scatter_(0, rows[full], gp[full])
+    assert torch.equal(G, ref)
+    return am
+
+
+@pytest.mark.parametrize("C", [70, 64])
+def test_segmax_unequal_segments(dev, C):
+    """CSR segments of unequal lengths, with empty and one-row segments, on an input with many ties."""
+    from superpoint_graph_b200 import ops
+    torch.manual_seed(11)
+    lens = torch.randint(0, 40, (41,))
+    lens[[0, 7, 40]] = 0
+    lens[[1, 2, 20]] = 1
+    seg = csr_seg(lens, dev)
+    Y = torch.round(torch.randn(int(lens.sum()), C, device=dev) * 4) / 4
+    check_pool_vs_torch(ops, Y, seg, C, dev)
+
+
+def check_segmax_bn_bwd(ops, Y, seg, C, dev):
+    """The fused max-pool + BatchNorm/ReLU backward against its unfused composition (segmax_bwd ->
+    act_bwd_reduce -> act_bwd_apply) over the same argmax."""
+    M = Y.shape[0]
+    eps = 1e-5
+    mean, var = Y.mean(0), Y.var(0, unbiased=False)
+    scale, shift = ops.bn_fold(mean, var, torch.rand(C, device=dev) + 0.5, torch.randn(C, device=dev), eps)
+    pooled = torch.empty(seg[0], C, device=dev)
+    am = ops.segmax_fwd(Y, C, seg, C, scale, shift, True, pooled, C)
+    gp = torch.randn(seg[0], C + 3, device=dev)  # unaligned pooled-gradient rows, as PointNet's
+    s1, s2, dY = ops.segmax_bn_bwd(gp, C + 3, am, Y, C, scale, shift, mean, var, eps, True, seg, C)
+    G = ops.segmax_bwd(gp, C + 3, am, seg, C)
+    s12 = ops.act_bwd_reduce(G, C, Y, C, scale, shift, mean, var, eps, True, M, C)
+    close(s1, s12[:C], 1e-5)
+    close(s2, s12[C:], 1e-5)
+    dY_ref = ops.act_bwd_apply(G, C, Y, C, scale, shift, mean, var, eps, True, True, s12[:C], s12[C:], M, C)
+    close(dY, dY_ref, 1e-5)
+
+
+@pytest.mark.parametrize("layout", ["fixed", "csr"])
+def test_segmax_bn_bwd(dev, layout):
+    from superpoint_graph_b200 import ops
+    torch.manual_seed(12)
+    B, L, C = 300, 24, 132
+    if layout == "fixed":
+        seg = (B, L, None, None)
+    else:
+        lens = torch.randint(0, 2 * L, (B,))
+        lens[[3, 150]] = 0
+        lens[[4, 151]] = 1
+        seg = csr_seg(lens, dev)
+    M = B * L if layout == "fixed" else int(seg[3].numel())
+    check_segmax_bn_bwd(ops, torch.randn(M, C, device=dev), seg, C, dev)
+
+
+def test_segmax_more_than_65535_segments(dev):
+    """Ragged pooling over more segments than one launch's grid.y holds, forward and backward."""
+    from superpoint_graph_b200 import ops
+    torch.manual_seed(13)
+    lens = torch.randint(0, 5, (70000,))
+    seg = csr_seg(lens, dev)
+    C = 64
+    Y = torch.round(torch.randn(int(lens.sum()), C, device=dev) * 4) / 4
+    check_pool_vs_torch(ops, Y, seg, C, dev)
+    check_segmax_bn_bwd(ops, torch.randn(int(lens.sum()), C, device=dev), seg, C, dev)
 
 
 def test_ce_loss_and_adam(dev):
