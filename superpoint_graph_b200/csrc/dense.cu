@@ -469,7 +469,9 @@ colstats_final_kernel(const float* __restrict__ ws, int64_t chunks, int C,
     }
 }
 
-// two-level driver; `partials` must have room for ceil(n/256) extra triples per column at its end
+// multi-level driver: every level folds 256 partials per block until one block is left, which
+// writes mean/var (and the fold).  `partials` must have room for ceil(n/256) extra triples per
+// column at its end; the levels alternate between that tail and the (consumed) front of `partials`.
 static int colstats_merge_launch(float* partials, int64_t n, int C, float* mean, float* var,
                                  cudaStream_t s, const FoldArgs& fold) {
     FoldArgs nofold;
@@ -479,22 +481,24 @@ static int colstats_merge_launch(float* partials, int64_t n, int C, float* mean,
     nofold.nbt = nullptr;
     nofold.eps = nofold.momentum = nofold.unbias = 0.f;
     const unsigned gx = (unsigned)ceil_div64(C, 32);
-    const int64_t P = ceil_div64(n, kMergePerBlock);
-    if (P > 65535) return SPG_E_UNSUPPORTED;
-    if (P == 1) {
-        SPG_LAUNCH(K_COLSTATS_FINAL, s, colstats_final_kernel, dim3(gx, 1), 1024, 0, partials, n, C,
-                   mean, var, (float*)nullptr, fold);
-        return launch_status();
+    float* const spare[2] = {partials + n * C * 3, partials};
+    float* src = partials;
+    for (int level = 0;; ++level) {
+        const int64_t P = ceil_div64(n, kMergePerBlock);
+        if (P == 1) {
+            SPG_LAUNCH(K_COLSTATS_FINAL, s, colstats_final_kernel, dim3(gx, 1), 1024, 0, src, n, C,
+                       mean, var, (float*)nullptr, fold);
+            return launch_status();
+        }
+        if (P > 65535) return SPG_E_UNSUPPORTED;
+        float* dst = spare[level & 1];
+        SPG_LAUNCH(K_COLSTATS_FINAL, s, colstats_final_kernel, dim3(gx, (unsigned)P), 1024, 0, src, n,
+                   C, mean, var, dst, nofold);
+        const int rc = launch_status();
+        if (rc) return rc;
+        src = dst;
+        n = P;
     }
-    float* lvl2 = partials + n * C * 3;
-    SPG_LAUNCH(K_COLSTATS_FINAL, s, colstats_final_kernel, dim3(gx, (unsigned)P), 1024, 0, partials, n,
-               C, mean, var, lvl2, nofold);
-    int rc = launch_status();
-    if (rc) return rc;
-    if (P > kMergePerBlock) return SPG_E_UNSUPPORTED;
-    SPG_LAUNCH(K_COLSTATS_FINAL, s, colstats_final_kernel, dim3(gx, 1), 1024, 0, lvl2, P, C, mean, var,
-               (float*)nullptr, fold);
-    return launch_status();
 }
 
 static FoldArgs no_fold() {
