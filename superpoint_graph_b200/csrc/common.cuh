@@ -22,7 +22,6 @@ enum KernelId {
     K_GRU_BWD,
     K_GEMM,
     K_GEMM_SPLITK_REDUCE,
-    K_COLSTATS_PARTIAL,
     K_COLSTATS_FINAL,
     K_BN_FOLD,
     K_AFFINE_ACT,
@@ -86,23 +85,52 @@ __device__ __forceinline__ void st_stream4(float4* p, float4 v) { __stcs(p, v); 
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.f / (1.f + expf(-v)); }
 
-// 128-bit vectorised variants (dense_vec.cu); return false if the shape/alignment does not fit.
-// slot != NULL: dropout with probability p (see spg_affine_act).
-bool vec_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy,
-                        const float* scale, const float* shift, const float* mean,
-                        const float* var, float eps, int relu, float* s12, float* ws,
-                        int64_t M, int C, float p, const int64_t* slot, cudaStream_t s, int* rc);
-bool vec_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float* ws,
-                cudaStream_t s, int* rc);
-bool vec_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
-                       const float* scale, const float* shift, const float* mean,
-                       const float* var, float eps, int relu, int has_bn, const float* s1,
-                       const float* s2, float* dY, int64_t lddy, int64_t M, int C, float p,
-                       const int64_t* slot, cudaStream_t s, int* rc);
-bool vec_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                    float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* slot,
-                    cudaStream_t s, int* rc);
-// out[c] = sum_k ws[k*C + c] for k < chunks (fp64, fixed order; dense_vec.cu), counted as kernel `kid`.
+// ---- BatchNorm/ReLU elements shared by the dense, max-pool and tensor-core kernels
+
+// Gradient through relu(y*sc + sh): g where the pre-activation is > 0, else 0 (NaN included).
+__device__ __forceinline__ float relu_bwd(float g, float y, float sc, float sh) {
+    return fmaf(y, sc, sh) > 0.f ? g : 0.f;
+}
+
+// BatchNorm backward of one element: sc*(g - s1/M - xhat*s2/M), xhat = (y - mu)*rstd, m1 = s1/M, m2 = s2/M.
+__device__ __forceinline__ float bn_bwd(float g, float y, float sc, float mu, float rstd, float m1, float m2) {
+    return sc * (g - m1 - (y - mu) * rstd * m2);
+}
+
+// BatchNorm fold of a column from its batch statistics: scale = gamma/sqrt(var+eps), shift =
+// beta - mean*scale, running = (1-momentum)*running + momentum*{mean, var*unbias}, nbt += 1.
+// gamma, beta, rmean, rvar and nbt may be NULL; `enabled` says whether a merge folds at all.
+struct FoldArgs {
+    const float *gamma, *beta;
+    float *scale, *shift, *rmean, *rvar;
+    long long* nbt;
+    float eps, momentum, unbias;
+    int enabled;
+};
+
+// unbias = M/(M-1) for a batch of M rows; enabled if scale != NULL
+inline FoldArgs fold_args(const float* gamma, const float* beta, float eps, float* scale, float* shift,
+                          float* rmean, float* rvar, int64_t* nbt, float momentum, int64_t M) {
+    FoldArgs f;
+    f.gamma = gamma; f.beta = beta; f.scale = scale; f.shift = shift;
+    f.rmean = rmean; f.rvar = rvar; f.nbt = (long long*)nbt;
+    f.eps = eps; f.momentum = momentum;
+    f.unbias = M > 1 ? (float)((double)M / (double)(M - 1)) : 1.f;
+    f.enabled = scale != nullptr;
+    return f;
+}
+
+__device__ __forceinline__ void bn_fold_col(const FoldArgs& f, int c, float mu, float var) {
+    const float rstd = 1.f / sqrtf(var + f.eps);
+    const float sc = (f.gamma ? f.gamma[c] : 1.f) * rstd;
+    f.scale[c] = sc;
+    f.shift[c] = (f.beta ? f.beta[c] : 0.f) - mu * sc;
+    if (f.rmean) f.rmean[c] = (1.f - f.momentum) * f.rmean[c] + f.momentum * mu;
+    if (f.rvar) f.rvar[c] = (1.f - f.momentum) * f.rvar[c] + f.momentum * var * f.unbias;
+    if (c == 0 && f.nbt) f.nbt[0] += 1;
+}
+
+// out[c] = sum_k ws[k*C + c] for k < chunks (fp64, fixed order; bn_act.cu), counted as kernel `kid`.
 int colsum_merge(int kid, const float* ws, int64_t chunks, int C, float* out, cudaStream_t s);
 
 }  // namespace spg

@@ -1,6 +1,7 @@
 // Dense fp32 building blocks of the PointNet / filter-network / classifier layers:
 // a tiled FMA GEMM with the producing layer's "BatchNorm apply + ReLU" fused into
-// the operand load, deterministic batch statistics, and the BatchNorm/ReLU backward.
+// the operand load, its split-K reduce, the merge of the batch statistics and the
+// BatchNorm fold.  The activation passes and column sums are in bn_act.cu.
 //
 // Reference semantics: nn.Conv1d(kernel 1) / nn.Linear / nn.BatchNorm1d / nn.ReLU as
 // stacked by learning/pointnet.py:27-53,83-118 and learning/graphnet.py:17-34.  The
@@ -12,7 +13,6 @@
 // small / odd shapes).  The large point-wise layers are served by the wgmma
 // 3xTF32 kernel in tc_gemm.cu when it applies.
 #include "common.cuh"
-#include "philox.cuh"
 
 namespace spg {
 
@@ -331,67 +331,12 @@ gemm_splitk_reduce_kernel(const float* __restrict__ ws, int split, int64_t M, in
     }
 }
 
-// ---------------------------------------------------------------- column reductions
-constexpr int kChunkRows = 1024;
-// the masked BatchNorm-backward sums spend a Philox call per element: shorter chunks, more CTAs
-constexpr int kDropChunkRows = 256;
-
-// per (chunk, column): count, mean, M2 (Welford), merged over the 8 row lanes (Chan).
-__global__ void __launch_bounds__(256)
-colstats_partial_kernel(const float* __restrict__ Y, int64_t ldy, int64_t M, int C,
-                        float* __restrict__ ws) {
-    SPG_PDL_ENTRY();
-    __shared__ float s_n[8][32], s_mean[8][32], s_m2[8][32];
-    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const int c = blockIdx.x * 32 + x;
-    const int64_t r0 = (int64_t)blockIdx.y * kChunkRows;
-    const int64_t r1 = min(M, r0 + kChunkRows);
-    float n = 0.f, mean = 0.f, m2 = 0.f;
-    if (c < C) {
-        for (int64_t r = r0 + y; r < r1; r += 8) {
-            const float v = __ldg(Y + r * ldy + c);
-            n += 1.f;
-            const float d = v - mean;
-            mean += d / n;
-            m2 = fmaf(d, v - mean, m2);
-        }
-    }
-    s_n[y][x] = n;
-    s_mean[y][x] = mean;
-    s_m2[y][x] = m2;
-    __syncthreads();
-    if (y == 0 && c < C) {
-        float na = s_n[0][x], ma = s_mean[0][x], qa = s_m2[0][x];
-        for (int j = 1; j < 8; ++j) {
-            const float nb = s_n[j][x], mb = s_mean[j][x], qb = s_m2[j][x];
-            if (nb > 0.f) {
-                const float nn = na + nb, d = mb - ma;
-                ma += d * (nb / nn);
-                qa += qb + d * d * (na * nb / nn);
-                na = nn;
-            }
-        }
-        float* o = ws + ((int64_t)blockIdx.y * C + c) * 3;
-        o[0] = na;
-        o[1] = ma;
-        o[2] = qa;
-    }
-}
-
 // Merge of (count, mean, M2) partials, deterministic and division-free in the inner loops:
 //   N = sum n_k, mean = sum n_k*mean_k / N, M2 = sum (M2_k + n_k*(mean_k - mean)^2)    (fp64 sums).
 // Block = 32 columns x 32 lanes, 256 partials per block (8 per thread, kept in registers between
 // the two passes); grid.y > 1 writes block-level partials (same triple format) for a second level.
+// The last level also executes the optional BatchNorm fold (saves a launch per layer).
 constexpr int kMergePerBlock = 256;
-
-// optional BatchNorm fold executed by the last merge level (saves a launch per layer)
-struct FoldArgs {
-    const float *gamma, *beta;
-    float *scale, *shift, *rmean, *rvar;
-    long long* nbt;
-    float eps, momentum, unbias;
-    int enabled;
-};
 
 __global__ void __launch_bounds__(1024)
 colstats_final_kernel(const float* __restrict__ ws, int64_t chunks, int C,
@@ -456,15 +401,7 @@ colstats_final_kernel(const float* __restrict__ ws, int64_t chunks, int C,
             const float var_f = ntot > 0.0 ? (float)(qq / ntot) : 0.f;
             mean[c] = mu_f;
             var[c] = var_f;
-            if (f.enabled) {
-                const float rstd = 1.f / sqrtf(var_f + f.eps);
-                const float sc = (f.gamma ? f.gamma[c] : 1.f) * rstd;
-                f.scale[c] = sc;
-                f.shift[c] = (f.beta ? f.beta[c] : 0.f) - mu_f * sc;
-                if (f.rmean) f.rmean[c] = (1.f - f.momentum) * f.rmean[c] + f.momentum * mu_f;
-                if (f.rvar) f.rvar[c] = (1.f - f.momentum) * f.rvar[c] + f.momentum * var_f * f.unbias;
-                if (c == 0 && f.nbt) f.nbt[0] += 1;
-            }
+            if (f.enabled) bn_fold_col(f, c, mu_f, var_f);
         }
     }
 }
@@ -474,12 +411,6 @@ colstats_final_kernel(const float* __restrict__ ws, int64_t chunks, int C,
 // column at its end; the levels alternate between that tail and the (consumed) front of `partials`.
 static int colstats_merge_launch(float* partials, int64_t n, int C, float* mean, float* var,
                                  cudaStream_t s, const FoldArgs& fold) {
-    FoldArgs nofold;
-    nofold.enabled = 0;
-    nofold.gamma = nofold.beta = nullptr;
-    nofold.scale = nofold.shift = nofold.rmean = nofold.rvar = nullptr;
-    nofold.nbt = nullptr;
-    nofold.eps = nofold.momentum = nofold.unbias = 0.f;
     const unsigned gx = (unsigned)ceil_div64(C, 32);
     float* const spare[2] = {partials + n * C * 3, partials};
     float* src = partials;
@@ -493,7 +424,7 @@ static int colstats_merge_launch(float* partials, int64_t n, int C, float* mean,
         if (P > 65535) return SPG_E_UNSUPPORTED;
         float* dst = spare[level & 1];
         SPG_LAUNCH(K_COLSTATS_FINAL, s, colstats_final_kernel, dim3(gx, (unsigned)P), 1024, 0, src, n,
-                   C, mean, var, dst, nofold);
+                   C, mean, var, dst, FoldArgs{});
         const int rc = launch_status();
         if (rc) return rc;
         src = dst;
@@ -501,174 +432,11 @@ static int colstats_merge_launch(float* partials, int64_t n, int C, float* mean,
     }
 }
 
-static FoldArgs no_fold() {
-    FoldArgs f;
-    f.enabled = 0;
-    f.gamma = f.beta = nullptr;
-    f.scale = f.shift = f.rmean = f.rvar = nullptr;
-    f.nbt = nullptr;
-    f.eps = f.momentum = f.unbias = 0.f;
-    return f;
-}
-
 __global__ void bn_fold_kernel(const float* __restrict__ mean, const float* __restrict__ var,
-                               const float* __restrict__ gamma, const float* __restrict__ beta,
-                               float eps, float* __restrict__ scale, float* __restrict__ shift,
-                               float* __restrict__ rmean, float* __restrict__ rvar,
-                               long long* __restrict__ nbt, float momentum, float unbias, int C) {
+                               const FoldArgs f, int C) {
     SPG_PDL_ENTRY();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c == 0 && nbt) nbt[0] += 1;
-    if (c >= C) return;
-    const float mu = mean[c], v = var[c];
-    const float rstd = 1.f / sqrtf(v + eps);
-    const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
-    const float sc = g * rstd;
-    scale[c] = sc;
-    shift[c] = b - mu * sc;
-    if (rmean) rmean[c] = (1.f - momentum) * rmean[c] + momentum * mu;
-    if (rvar) rvar[c] = (1.f - momentum) * rvar[c] + momentum * v * unbias;
-}
-
-// DROP (here and in the act_bwd kernels): dropout with probability p, mask from `slot` (philox.cuh)
-template <bool DROP>
-__global__ void __launch_bounds__(256)
-affine_act_kernel(const float* __restrict__ Y, int64_t ldy, const float* __restrict__ scale,
-                  const float* __restrict__ shift, int relu, float* __restrict__ out, int64_t ldo,
-                  int64_t M, int C, float p, const int64_t* __restrict__ slot) {
-    SPG_PDL_ENTRY();
-    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const int c = blockIdx.x * 32 + x;
-    if (c >= C) return;
-    const float sc = scale ? scale[c] : 1.f, sh = shift ? shift[c] : 0.f;
-    const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
-    for (int64_t r = (int64_t)blockIdx.y * 8 + y; r < M; r += (int64_t)gridDim.y * 8) {
-        float v = fmaf(Y[r * ldy + c], sc, sh);
-        if (relu) v = fmaxf(v, 0.f);
-        if constexpr (DROP) v = drop_at(d, r * C + c, v);
-        out[r * ldo + c] = v;
-    }
-}
-
-__global__ void __launch_bounds__(256)
-colsum_partial_kernel(const float* __restrict__ X, int64_t ldx, int64_t M, int C,
-                      float* __restrict__ ws) {
-    SPG_PDL_ENTRY();
-    __shared__ float s[8][32];
-    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const int c = blockIdx.x * 32 + x;
-    const int64_t r0 = (int64_t)blockIdx.y * kChunkRows;
-    const int64_t r1 = min(M, r0 + kChunkRows);
-    float a = 0.f;
-    if (c < C)
-        for (int64_t r = r0 + y; r < r1; r += 8) a += __ldg(X + r * ldx + c);
-    s[y][x] = a;
-    __syncthreads();
-    if (y == 0 && c < C) {
-        float t = 0.f;
-        for (int j = 0; j < 8; ++j) t += s[j][x];
-        ws[(int64_t)blockIdx.y * C + c] = t;
-    }
-}
-
-// out[c] = sum over chunks of ws[k*stride + c*inner + off] accumulated in double.
-__global__ void colsum_final_kernel(const float* __restrict__ ws, int64_t chunks, int C,
-                                    float* __restrict__ out) {
-    SPG_PDL_ENTRY();
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    double a = 0.0;
-    for (int64_t k = 0; k < chunks; ++k) a += (double)ws[k * C + c];
-    out[c] = (float)a;
-}
-
-template <bool DROP>
-__global__ void __launch_bounds__(256)
-act_bwd_reduce_kernel(const float* __restrict__ G, int64_t ldg, const float* __restrict__ Y,
-                      int64_t ldy, const float* __restrict__ scale,
-                      const float* __restrict__ shift, const float* __restrict__ mean,
-                      const float* __restrict__ var, float eps, int relu, float* __restrict__ ws,
-                      int64_t M, int C, float p, const int64_t* __restrict__ slot) {
-    SPG_PDL_ENTRY();
-    __shared__ float s1[8][32], s2[8][32];
-    constexpr int kRows = DROP ? kDropChunkRows : kChunkRows;
-    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const int c = blockIdx.x * 32 + x;
-    const int64_t r0 = (int64_t)blockIdx.y * kRows;
-    const int64_t r1 = min(M, r0 + kRows);
-    float a1 = 0.f, a2 = 0.f;
-    if (c < C) {
-        const float sc = scale[c], sh = shift[c], mu = mean[c];
-        const float rstd = 1.f / sqrtf(var[c] + eps);
-        const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
-        for (int64_t r = r0 + y; r < r1; r += 8) {
-            const float yv = __ldg(Y + r * ldy + c);
-            float g = __ldg(G + r * ldg + c);
-            if constexpr (DROP) g = drop_at(d, r * C + c, g);
-            if (relu && !(fmaf(yv, sc, sh) > 0.f)) g = 0.f;
-            a1 += g;
-            a2 = fmaf(g, (yv - mu) * rstd, a2);
-        }
-    }
-    s1[y][x] = a1;
-    s2[y][x] = a2;
-    __syncthreads();
-    if (y == 0 && c < C) {
-        float t1 = 0.f, t2 = 0.f;
-        for (int j = 0; j < 8; ++j) {
-            t1 += s1[j][x];
-            t2 += s2[j][x];
-        }
-        ws[((int64_t)blockIdx.y * 2) * C + c] = t1;
-        ws[((int64_t)blockIdx.y * 2 + 1) * C + c] = t2;
-    }
-}
-
-__global__ void act_bwd_reduce_final_kernel(const float* __restrict__ ws, int64_t chunks, int C,
-                                            float* __restrict__ s1, float* __restrict__ s2) {
-    SPG_PDL_ENTRY();
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    double a1 = 0.0, a2 = 0.0;
-    for (int64_t k = 0; k < chunks; ++k) {
-        a1 += (double)ws[(k * 2) * C + c];
-        a2 += (double)ws[(k * 2 + 1) * C + c];
-    }
-    s1[c] = (float)a1;
-    s2[c] = (float)a2;
-}
-
-template <bool DROP>
-__global__ void __launch_bounds__(256)
-act_bwd_apply_kernel(const float* __restrict__ G, int64_t ldg, const float* __restrict__ Y,
-                     int64_t ldy, const float* __restrict__ scale, const float* __restrict__ shift,
-                     const float* __restrict__ mean, const float* __restrict__ var, float eps,
-                     int relu, int has_bn, const float* __restrict__ s1,
-                     const float* __restrict__ s2, float* __restrict__ dY, int64_t lddy, int64_t M,
-                     int C, float p, const int64_t* __restrict__ slot) {
-    SPG_PDL_ENTRY();
-    const int x = threadIdx.x & 31, y = threadIdx.x >> 5;
-    const int c = blockIdx.x * 32 + x;
-    if (c >= C) return;
-    const float sc = (has_bn || scale) ? (scale ? scale[c] : 1.f) : 1.f;
-    const float sh = shift ? shift[c] : 0.f;
-    float mu = 0.f, rstd = 1.f, m1 = 0.f, m2 = 0.f;
-    if (has_bn) {
-        mu = mean[c];
-        rstd = 1.f / sqrtf(var[c] + eps);
-        m1 = s1[c] / (float)M;
-        m2 = s2[c] / (float)M;
-    }
-    const DropParams d = DROP ? drop_params(slot, p) : DropParams{};
-    for (int64_t r = (int64_t)blockIdx.y * 8 + y; r < M; r += (int64_t)gridDim.y * 8) {
-        const float yv = Y ? Y[r * ldy + c] : 0.f;
-        float g = G[r * ldg + c];
-        if constexpr (DROP) g = drop_at(d, r * C + c, g);
-        if (relu && !(fmaf(yv, sc, sh) > 0.f)) g = 0.f;
-        float d = g;
-        if (has_bn) d = sc * (g - m1 - (yv - mu) * rstd * m2);
-        dY[r * lddy + c] = d;
-    }
+    if (c < C) bn_fold_col(f, c, mean[c], var[c]);
 }
 
 static inline bool a16(const void* p) { return ((uintptr_t)p & 15) == 0; }
@@ -747,7 +515,6 @@ int spg_gemm(const float* A, int64_t lda, int a_kmajor, const float* B, int64_t 
     return SPG_OK;
 }
 
-// workspace bound for the column reductions (the vectorised kernels use 256-row chunks)
 int spg_splitk_reduce(const float* partials, int split, int64_t M, int64_t N, const float* bias,
                       float* C, int64_t ldc, spg_stream_t stream) {
     if (!partials || !C || split < 1 || M <= 0 || N <= 0 || ldc < N) return SPG_E_BADARG;
@@ -757,29 +524,15 @@ int spg_splitk_reduce(const float* partials, int split, int64_t M, int64_t N, co
     return launch_status();
 }
 
+// workspace bound of the column reductions (bn_act.cu): 256-row chunks at most
 int64_t spg_colstats_chunks(int64_t M) { return M <= 0 ? 1 : ceil_div64(M, 256); }
-static inline int64_t scalar_chunks(int64_t M) { return M <= 0 ? 1 : ceil_div64(M, kChunkRows); }
-
-int spg_colstats(const float* Y, int64_t ldy, int64_t M, int C, float* mean, float* var,
-                 float* workspace, spg_stream_t stream) {
-    if (M <= 0 || C <= 0 || !Y || !mean || !var || !workspace || ldy < C) return SPG_E_BADARG;
-    const int64_t chunks = scalar_chunks(M);
-    if (chunks > 65535) return SPG_E_UNSUPPORTED;
-    cudaStream_t s = (cudaStream_t)stream;
-    dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)chunks);
-    SPG_LAUNCH(K_COLSTATS_PARTIAL, s, colstats_partial_kernel, grid, 256, 0, Y, ldy, M, C,
-               workspace);
-    int rc = launch_status();
-    if (rc) return rc;
-    return colstats_merge_launch(workspace, chunks, C, mean, var, s, no_fold());
-}
 
 int64_t spg_gemm_stats_tiles(int64_t M) { return M <= 0 ? 1 : ceil_div64(M, BM); }
 
 int spg_colstats_merge(float* partials, int64_t n_partials, int C, float* mean, float* var,
                        spg_stream_t stream) {
     if (n_partials <= 0 || C <= 0 || !partials || !mean || !var) return SPG_E_BADARG;
-    return colstats_merge_launch(partials, n_partials, C, mean, var, (cudaStream_t)stream, no_fold());
+    return colstats_merge_launch(partials, n_partials, C, mean, var, (cudaStream_t)stream, FoldArgs{});
 }
 
 int spg_colstats_merge_fold(float* partials, int64_t n_partials, int C, float* mean, float* var,
@@ -788,13 +541,9 @@ int spg_colstats_merge_fold(float* partials, int64_t n_partials, int C, float* m
                             int64_t* num_batches_tracked, float momentum, int64_t M,
                             spg_stream_t stream) {
     if (n_partials <= 0 || C <= 0 || !partials || !mean || !var || !scale || !shift) return SPG_E_BADARG;
-    FoldArgs f;
-    f.enabled = 1;
-    f.gamma = gamma; f.beta = beta; f.scale = scale; f.shift = shift;
-    f.rmean = running_mean; f.rvar = running_var; f.nbt = (long long*)num_batches_tracked;
-    f.eps = eps; f.momentum = momentum;
-    f.unbias = M > 1 ? (float)((double)M / (double)(M - 1)) : 1.f;
-    return colstats_merge_launch(partials, n_partials, C, mean, var, (cudaStream_t)stream, f);
+    return colstats_merge_launch(partials, n_partials, C, mean, var, (cudaStream_t)stream,
+                                 fold_args(gamma, beta, eps, scale, shift, running_mean, running_var,
+                                           num_batches_tracked, momentum, M));
 }
 
 int spg_bn_fold(const float* mean, const float* var, const float* gamma, const float* beta,
@@ -802,112 +551,11 @@ int spg_bn_fold(const float* mean, const float* var, const float* gamma, const f
                 int64_t* num_batches_tracked, float momentum, int64_t M, int C,
                 spg_stream_t stream) {
     if (C <= 0 || !mean || !var || !scale || !shift) return SPG_E_BADARG;
-    const float unbias = M > 1 ? (float)((double)M / (double)(M - 1)) : 1.f;
     SPG_LAUNCH(K_BN_FOLD, (cudaStream_t)stream, bn_fold_kernel, (unsigned)ceil_div64(C, 128), 128,
-               0, mean, var, gamma, beta, eps, scale, shift, running_mean, running_var,
-               (long long*)num_batches_tracked, momentum, unbias, C);
-    return launch_status();
-}
-
-// CTAs along the rows of the element-wise passes; the masked (DROP) passes are bound by the Philox
-// latency, not by bandwidth: one row step per thread where the cap allows.
-static inline unsigned rows_grid(int64_t M, bool drop) {
-    int64_t g = ceil_div64(M, drop ? 8 : 64);
-    if (g > 8 * kNumSMs) g = 8 * kNumSMs;
-    if (g < 1) g = 1;
-    return (unsigned)g;
-}
-
-int spg_affine_act(const float* Y, int64_t ldy, const float* scale, const float* shift, int relu,
-                   float* out, int64_t ldo, int64_t M, int C, float p, const int64_t* drop_slot,
-                   spg_stream_t stream) {
-    if (M < 0 || C <= 0 || (drop_slot && !(p >= 0.f))) return SPG_E_BADARG;
-    if (M == 0) return SPG_OK;
-    if (!Y || !out || ldy < C || ldo < C) return SPG_E_BADARG;
-    {
-        int rc = 0;
-        if (vec_affine_act(Y, ldy, scale, shift, relu, out, ldo, M, C, p, drop_slot,
-                           (cudaStream_t)stream, &rc))
-            return rc;
-    }
-    const bool drop = drop_slot != nullptr;
-    dim3 grid((unsigned)ceil_div64(C, 32), rows_grid(M, drop));
-    SPG_LAUNCH(drop ? K_DROPOUT_FWD : K_AFFINE_ACT, (cudaStream_t)stream,
-               (drop ? affine_act_kernel<true> : affine_act_kernel<false>), grid, 256, 0, Y, ldy,
-               scale, shift, relu, out, ldo, M, C, p, drop_slot);
-    return launch_status();
-}
-
-int spg_colsum(const float* X, int64_t ldx, int64_t M, int C, float* out, float* workspace,
-               spg_stream_t stream) {
-    if (M <= 0 || C <= 0 || !X || !out || !workspace || ldx < C) return SPG_E_BADARG;
-    {
-        int rc = 0;
-        if (vec_colsum(X, ldx, M, C, out, workspace, (cudaStream_t)stream, &rc)) return rc;
-    }
-    const int64_t chunks = scalar_chunks(M);
-    if (chunks > 65535) return SPG_E_UNSUPPORTED;
-    cudaStream_t s = (cudaStream_t)stream;
-    dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)chunks);
-    SPG_LAUNCH(K_COLSUM_PARTIAL, s, colsum_partial_kernel, grid, 256, 0, X, ldx, M, C, workspace);
-    int rc = launch_status();
-    if (rc) return rc;
-    SPG_LAUNCH(K_COLSUM_FINAL, s, colsum_final_kernel, (unsigned)ceil_div64(C, 128), 128, 0,
-               workspace, chunks, C, out);
-    return launch_status();
-}
-
-int spg_act_bwd_reduce(const float* G, int64_t ldg, const float* Y, int64_t ldy,
-                       const float* scale, const float* shift, const float* mean,
-                       const float* var, float eps, int relu, float* s12, float* workspace,
-                       int64_t M, int C, float p, const int64_t* drop_slot, spg_stream_t stream) {
-    if (M <= 0 || C <= 0 || !G || !Y || !scale || !shift || !mean || !var || !s12 ||
-        !workspace || (drop_slot && !(p >= 0.f)))
-        return SPG_E_BADARG;
-    {
-        int rc = 0;
-        if (vec_act_bwd_reduce(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, s12, workspace,
-                               M, C, p, drop_slot, (cudaStream_t)stream, &rc))
-            return rc;
-    }
-    const bool drop = drop_slot != nullptr;
-    const int64_t chunks = drop ? ceil_div64(M, kDropChunkRows) : scalar_chunks(M);
-    if (chunks > 65535) return SPG_E_UNSUPPORTED;
-    cudaStream_t s = (cudaStream_t)stream;
-    dim3 grid((unsigned)ceil_div64(C, 32), (unsigned)chunks);
-    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE : K_ACT_BWD_REDUCE, s,
-               (drop ? act_bwd_reduce_kernel<true> : act_bwd_reduce_kernel<false>), grid, 256, 0,
-               G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, workspace, M, C, p, drop_slot);
-    int rc = launch_status();
-    if (rc) return rc;
-    SPG_LAUNCH(drop ? K_DROPOUT_BWD_REDUCE_FINAL : K_ACT_BWD_REDUCE_FINAL, s,
-               act_bwd_reduce_final_kernel, (unsigned)ceil_div64(C, 128), 128, 0, workspace, chunks,
-               C, s12, s12 + C);
-    return launch_status();
-}
-
-int spg_act_bwd_apply(const float* G, int64_t ldg, const float* Y, int64_t ldy,
-                      const float* scale, const float* shift, const float* mean,
-                      const float* var, float eps, int relu, int has_bn, const float* s1,
-                      const float* s2, float* dY, int64_t lddy, int64_t M, int C, float p,
-                      const int64_t* drop_slot, spg_stream_t stream) {
-    if (M < 0 || C <= 0 || (drop_slot && !(p >= 0.f))) return SPG_E_BADARG;
-    if (M == 0) return SPG_OK;
-    if (!G || !dY) return SPG_E_BADARG;
-    if ((relu || has_bn) && !Y) return SPG_E_BADARG;
-    if (has_bn && (!scale || !shift || !mean || !var || !s1 || !s2)) return SPG_E_BADARG;
-    {
-        int rc = 0;
-        if (vec_act_bwd_apply(G, ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2,
-                              dY, lddy, M, C, p, drop_slot, (cudaStream_t)stream, &rc))
-            return rc;
-    }
-    const bool drop = drop_slot != nullptr;
-    dim3 grid((unsigned)ceil_div64(C, 32), rows_grid(M, drop));
-    SPG_LAUNCH(drop ? K_DROPOUT_BWD_APPLY : K_ACT_BWD_APPLY, (cudaStream_t)stream,
-               (drop ? act_bwd_apply_kernel<true> : act_bwd_apply_kernel<false>), grid, 256, 0, G,
-               ldg, Y, ldy, scale, shift, mean, var, eps, relu, has_bn, s1, s2, dY, lddy, M, C, p,
-               drop_slot);
+               0, mean, var,
+               fold_args(gamma, beta, eps, scale, shift, running_mean, running_var,
+                         num_batches_tracked, momentum, M),
+               C);
     return launch_status();
 }
 

@@ -8,8 +8,8 @@
 // of storing it.  (seed, ctr) live in device memory: spg_dropout_rng_next copies the device generator state
 // into a per-site slot and advances the counter, every other kernel reads the slot — nothing about the stream
 // position is baked into launch parameters, so replays of a captured CUDA graph draw fresh masks.
-// The masked forward and backward are the DROP instantiations of the activation kernels (dense.cu,
-// dense_vec.cu); this file holds the slot kernel and the mask export.
+// The masked forward and backward are the DROP instantiations of the activation kernels
+// (bn_act.cu); this file holds the slot kernel and the mask export.
 #include "common.cuh"
 #include "philox.cuh"
 

@@ -258,7 +258,7 @@ segmax_bn_bwd_reduce_kernel(const float* __restrict__ gp, int64_t ldg, const int
             if (Segs::kMayBeEmpty && l < 0) continue;  // empty segment: no row, no gradient
             const float yv = __ldg(Y + (segs.begin(b) + l) * ldy + c);
             float g = __ldg(gp + b * ldg + c);
-            if (relu && !(fmaf(yv, sc, sh) > 0.f)) g = 0.f;
+            if (relu) g = relu_bwd(g, yv, sc, sh);
             a1 += g;
             a2 = fmaf(g, (yv - mu) * rstd, a2);
         }
@@ -316,8 +316,8 @@ segmax_bn_bwd_apply_kernel(const float* __restrict__ gp, int64_t ldg, const int*
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             float g = (aq[j] == l) ? gv[j] : 0.f;
-            if (relu && !(fmaf(yv[j], sc[j], sh[j]) > 0.f)) g = 0.f;
-            d[j] = sc[j] * (g - m1[j] - (yv[j] - mu[j]) * rs[j] * m2[j]);
+            if (relu) g = relu_bwd(g, yv[j], sc[j], sh[j]);
+            d[j] = bn_bwd(g, yv[j], sc[j], mu[j], rs[j], m1[j], m2[j]);
         }
         *reinterpret_cast<float4*>(dY + r * lddy + c) = make_float4(d[0], d[1], d[2], d[3]);
     }

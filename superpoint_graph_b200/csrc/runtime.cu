@@ -13,7 +13,7 @@ static const char* kKernelNames[K_COUNT] = {
     "ecc_vv_fwd",        "ecc_mat_fwd",        "ecc_generic_fwd",     "ecc_vv_bwd_w",
     "ecc_mat_bwd_w",     "ecc_generic_bwd_w",  "ecc_vv_bwd_x",        "ecc_mat_bwd_x",
     "ecc_generic_bwd_x", "gru_cell_fwd",       "gru_cell_bwd",        "gemm_f32",
-    "gemm_splitk_reduce", "colstats_partial",  "colstats_final",      "bn_fold",
+    "gemm_splitk_reduce", "colstats_final",    "bn_fold",
     "affine_act",        "colsum_partial",     "colsum_final",        "act_bwd_reduce",
     "act_bwd_reduce_final", "act_bwd_apply",   "cloud_rows",          "segmax_fwd",
     "segmax_bwd",        "stn_apply_bwd",      "rows_scatter",        "rows_gather",

@@ -71,11 +71,7 @@ struct Tc2Args {
     float* part;    // per-CTA partials [gridDim.x][N][3 | 2]
     // EPI_STATS outputs (+ optional fold)
     float *mean_out, *var_out;
-    const float *gamma, *beta;
-    float *scale_out, *shift_out, *rmean, *rvar;
-    long long* nbt;
-    float eps, momentum, unbias;
-    int fold;
+    FoldArgs fold;
     // EPI_BNRED inputs (layer below) and output
     const float* e_y;
     int64_t e_ldy;
@@ -500,15 +496,7 @@ __global__ void __launch_bounds__(256) tc_merge_kernel(const Tc2Args p, int P) {
                 const float var_f = sn > 0.0 ? (float)(qq / sn) : 0.f;
                 p.mean_out[c] = mu_f;
                 p.var_out[c] = var_f;
-                if (p.fold) {
-                    const float rstd = 1.f / sqrtf(var_f + p.eps);
-                    const float sc = (p.gamma ? p.gamma[c] : 1.f) * rstd;
-                    p.scale_out[c] = sc;
-                    p.shift_out[c] = (p.beta ? p.beta[c] : 0.f) - mu_f * sc;
-                    if (p.rmean) p.rmean[c] = (1.f - p.momentum) * p.rmean[c] + p.momentum * mu_f;
-                    if (p.rvar) p.rvar[c] = (1.f - p.momentum) * p.rvar[c] + p.momentum * var_f * p.unbias;
-                    if (c == 0 && p.nbt) p.nbt[0] += 1;
-                }
+                if (p.fold.enabled) bn_fold_col(p.fold, c, mu_f, var_f);
             }
         } else {
             double a1 = 0.0, a2 = 0.0;
@@ -643,11 +631,9 @@ int spg_tc_gemm_ex(const float* A, int64_t lda, const float* weight_image, const
     a.a_mean = a_mean; a.a_var = a_var; a.a_s12 = a_s12; a.a_eps = a_eps;
     a.dy_out = dy_out; a.lddy = lddy;
     a.epi = epilogue; a.part = partials_ws;
-    a.mean_out = mean_out; a.var_out = var_out; a.gamma = gamma; a.beta = beta;
-    a.scale_out = scale_out; a.shift_out = shift_out; a.rmean = running_mean; a.rvar = running_var;
-    a.nbt = (long long*)num_batches_tracked; a.eps = eps; a.momentum = momentum;
-    a.unbias = M > 1 ? (float)((double)M / (double)(M - 1)) : 1.f;
-    a.fold = scale_out != nullptr;
+    a.mean_out = mean_out; a.var_out = var_out;
+    a.fold = fold_args(gamma, beta, eps, scale_out, shift_out, running_mean, running_var, num_batches_tracked,
+                       momentum, M);
     a.e_y = e_y; a.e_ldy = e_ldy; a.e_scale = e_scale; a.e_shift = e_shift; a.e_mean = e_mean;
     a.e_var = e_var; a.e_eps = e_eps; a.e_relu = e_relu; a.e_s12 = e_s12; a.nstages = 0;
     const bool bnbwd = a2 != nullptr;
@@ -656,7 +642,7 @@ int spg_tc_gemm_ex(const float* A, int64_t lda, const float* weight_image, const
     if (dy_out && (!bnbwd || (lddy & 3) || lddy < K)) return SPG_E_BADARG;
     if (epilogue == EPI_STATS) {
         if (!partials_ws || !mean_out || !var_out) return SPG_E_BADARG;
-        if (a.fold && !shift_out) return SPG_E_BADARG;
+        if (a.fold.enabled && !shift_out) return SPG_E_BADARG;
     } else if (epilogue == EPI_BNRED) {
         if (!partials_ws || !e_y || !e_mean || !e_var || !e_s12 || (e_ldy & 3) || e_ldy < N) return SPG_E_BADARG;
     } else if (epilogue != EPI_NONE) {

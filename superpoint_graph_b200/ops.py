@@ -510,15 +510,6 @@ def _chunks(M):
     return max(1, (M + 255) // 256)
 
 
-def colstats(Y, ldy, M, C):
-    _need_cuda(Y)
-    mean = torch.empty(C, dtype=torch.float32, device=Y.device)
-    var = torch.empty(C, dtype=torch.float32, device=Y.device)
-    ws = workspace(3 * C * (_chunks(M) + _chunks(M) // 256 + 2), Y.device)
-    _lib.call("spg_colstats", Y, ldy, M, C, mean, var, ws, _lib.current_stream())
-    return mean, var
-
-
 def bn_fold(mean, var, gamma, beta, eps, running_mean=None, running_var=None, momentum=0.1, M=0,
             num_batches_tracked=None):
     _need_cuda(mean, var)

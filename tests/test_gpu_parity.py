@@ -236,16 +236,16 @@ def test_gemm_prologues_and_reduction(dev):
 
 
 @pytest.mark.parametrize("M,C", [(5000, 70), (4999, 64), (1031, 32), (777, 16), (3000, 96), (2500, 256)])
-def test_batch_stats_and_bn_backward(dev, M, C):
-    """C = 70: scalar kernels; C % 4 == 0: 128-bit kernels, with the warp folded over several rows
-    for the narrow power-of-two widths (64, 32, 16) and spanning 128 columns otherwise."""
+def test_colsum_bn_fold_and_bn_backward(dev, M, C):
+    """Column sums, the BatchNorm fold and running statistics, the BatchNorm/ReLU forward and backward
+    against nn.BatchNorm1d, from batch statistics computed in float64.  C = 70: one float per lane
+    (V = 1); C % 4 == 0: V = 4, with the warp folded over several rows for the narrow power-of-two
+    widths (64, 32, 16) and spanning 128 columns otherwise."""
     from superpoint_graph_b200 import ops
     torch.manual_seed(2)
     Y = (torch.randn(M, C, dtype=torch.float64) * 3 + 100)  # large mean: cancellation-prone
     Yf = Y.float().to(dev)
-    mean, var = ops.colstats(Yf, C, M, C)
-    close(mean, Yf.double().mean(0), 1e-6)
-    close(var, Yf.double().var(0, unbiased=False), 1e-5)
+    mean, var = Yf.double().mean(0).float(), Yf.double().var(0, unbiased=False).float()
     close(ops.colsum(Yf, C, M, C), Yf.double().sum(0), 1e-6)
     gamma, beta = torch.rand(C, device=dev) + 0.5, torch.randn(C, device=dev)
     gamma[::4] *= -1
@@ -270,6 +270,52 @@ def test_batch_stats_and_bn_backward(dev, M, C):
     close(s2, bn.weight.grad, 1e-4, 1e-4)
     dY = ops.act_bwd_apply(G, C, Yf, C, scale, shift, mean, var, 1e-5, True, True, s1, s2, M, C)
     close(dY, Yr.grad, 1e-4, 1e-6)
+
+
+@pytest.mark.parametrize("C", [16, 64])
+@pytest.mark.parametrize("p", [None, 0.3])
+@pytest.mark.parametrize("force", ["ld", "offset"])
+def test_bn_act_one_float_per_lane_at_widths_divisible_by_4(dev, C, p, force):
+    """A leading dimension of C + 1 or a pointer one float off 16 bytes runs the V = 1 kernels at
+    C % 4 == 0.  affine_act and act_bwd_apply give the bits of the V = 4 kernels on the same data;
+    act_bwd_reduce and colsum match float64."""
+    from superpoint_graph_b200 import ops
+    torch.manual_seed(5)
+    M, eps = 3001, 1e-5
+
+    def v1(X):  # the values of X in a layout that only V = 1 accepts: (tensor, leading dimension)
+        if force == "ld":
+            P = torch.full((M, C + 1), float("nan"), device=dev)
+            P[:, :C] = X
+            return P, C + 1
+        return torch.empty(M * C + 1, device=dev)[1:].view(M, C).copy_(X), C
+
+    Y = torch.randn(M, C, device=dev) * 2 + 0.5
+    G = torch.randn(M, C, device=dev)
+    (Y1, ld1), (G1, _) = v1(Y), v1(G)
+    scale, shift = torch.rand(C, device=dev) + 0.5, torch.randn(C, device=dev)
+    mean, var = Y.double().mean(0).float(), Y.double().var(0, unbiased=False).float()
+    drop = None if p is None else (p, torch.tensor([0x5EED, 17], dtype=torch.int64, device=dev))
+
+    a4 = ops.affine_act(Y, C, M, C, scale, shift, True, drop=drop)
+    assert torch.equal(ops.affine_act(Y1, ld1, M, C, scale, shift, True, drop=drop), a4)
+    close(ops.colsum(Y1, ld1, M, C), Y.double().sum(0), 1e-6)
+
+    s12 = ops.act_bwd_reduce(G1, ld1, Y1, ld1, scale, shift, mean, var, eps, True, M, C, drop=drop)
+    g = G.double()
+    if drop is not None:
+        g = g * ops.dropout_mask(drop[1], p, M, C).double() / (1 - np.float32(p))
+    Yd = Y.double()
+    g = g * (Yd * scale.double() + shift.double() > 0)
+    xhat = (Yd - mean.double()) / torch.sqrt(var.double() + np.float32(eps))
+    close(s12[:C], g.sum(0), 1e-4, 1e-5)
+    close(s12[C:], (g * xhat).sum(0), 1e-4, 1e-4)
+
+    s1, s2 = s12[:C], s12[C:]
+    d4 = ops.act_bwd_apply(G, C, Y, C, scale, shift, mean, var, eps, True, True, s1, s2, M, C, drop=drop)
+    d1 = ops.act_bwd_apply(G1, ld1, Y1, ld1, scale, shift, mean, var, eps, True, True, s1, s2, M, C,
+                           drop=drop)
+    assert torch.equal(d1, d4)
 
 
 def csr_seg(lens, dev):

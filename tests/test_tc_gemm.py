@@ -8,7 +8,7 @@ kernel by kernel and compared with float64 references computed on the CPU from t
   * dense.cu: spg_gemm with fused batch statistics, including a problem taller than one launch.
 
 Every product is 3xTF32 or fp32, i.e. fp32-equivalent (DESIGN §3: ~1e-6 relative).  The bounds are
-1e-5 of the tensor maximum; means 1e-6 and variances 1e-5, as in test_batch_stats_and_bn_backward.  The
+1e-5 of the tensor maximum; means 1e-6 and variances 1e-5.  The
 data are mean-zero, so a skipped or duplicated 32-row chunk or 128-row tile moves a result by ~1e-2
 relative, far above the bounds.  Every case draws from its own seed.
 
