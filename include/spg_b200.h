@@ -100,6 +100,38 @@ int spg_ecc_bwd_x(const void* w, const void* g, const int32_t* tgt_rowptr,
                   int64_t n_in, int64_t n_edges, int c_in, int c_out, int w_is_matrix,
                   int dtype, spg_stream_t stream);
 
+/* ------------------------------------------------------------ ECC-CRF  */
+/* The mean-field recurrence of ECC_CRFModule over a square graph (n nodes, n_in == n_out),
+ * float32, matrix filters w [n_edges,C,C] with 1 <= C <= 32, no idxe.
+ *   Q_0 = softmax(U);  Z_r = U - P_r,  P_r[t] = (1/deg_t) sum_{e in in(t)} Q_{r-1}[idxn_e] @ w[e];
+ *   Q_r = softmax(Z_r) for r < R;  the module returns Z_R.
+ * ref: learning/modules.py:185-202 (ECC_CRFModule.forward), graphnet.py:57-64.       */
+
+/* out = softmax(x) over each row of x [n,C]  (g == NULL), or
+ * out = x * (g - <g,x>) row by row, the softmax backward with x = softmax output (g != NULL).
+ * ref: modules.py:196,201 (nnf.softmax on 2-D input, dim 1).                       */
+int spg_crf_softmax(const float* x, const float* g, float* out, int64_t n, int C,
+                    spg_stream_t stream);
+
+/* One forward iteration: out[t] = softmax(Z_r[t]) if do_softmax else Z_r[t], with Z_r as above from
+ * U [n,C] and q_prev = Q_{r-1} [n,C]; a warp per target, filters read once, no atomics.
+ * ref: modules.py:197-201 (propagation, `input - Q`, softmax).                       */
+int spg_crf_fwd_step(const float* u, const float* q_prev, const float* w, const int32_t* tgt_rowptr,
+                     const int32_t* idxn, float* out, int64_t n, int64_t n_edges, int C,
+                     int do_softmax, spg_stream_t stream);
+
+/* One backward iteration over the SOURCE CSR (a warp per source row, no atomics), from
+ * gp = dL/dP_r = -dL/dZ_r [n,C]:
+ *   dQ[j]  = sum_{e: idxn_e = j} w[e] @ gp[tgt_e] / deg_tgt
+ *   dZ[j]  = q_prev[j] * (dQ[j] - <dQ[j], q_prev[j]>)          (q_prev = Q_{r-1})
+ *   du_out[j] = du_in[j] + dZ[j]    (du_out may alias du_in)
+ *   gp_out[j] = -dZ[j]              (gp_out = dL/dP_{r-1}; NULL skips it)
+ * ref: the autograd of modules.py:197-201 and GraphConvModule.py:135-146.            */
+int spg_crf_bwd_step(const float* w, const float* gp, const float* q_prev,
+                     const float* du_in, float* du_out, float* gp_out, const int32_t* tgt_rowptr,
+                     const int32_t* src_rowptr, const int32_t* src_perm, const int32_t* edge_tgt,
+                     int64_t n, int64_t n_edges, int C, spg_stream_t stream);
+
 
 /* ----------------------------------------------------------- GRUCellEx    */
 #define SPG_GRU_LAYERNORM 1

@@ -55,6 +55,9 @@ enum KernelId {
     K_DROPOUT_BWD_REDUCE,
     K_DROPOUT_BWD_REDUCE_FINAL,
     K_DROPOUT_BWD_APPLY,
+    K_CRF_FWD,
+    K_CRF_BWD,
+    K_CRF_SOFTMAX,
     K_COUNT
 };
 

@@ -23,6 +23,7 @@ static const char* kKernelNames[K_COUNT] = {
     "pointnet_fused_eval", "graph_build",
     "dropout_rng_next",  "dropout_fwd",        "dropout_mask",        "dropout_bwd_reduce",
     "dropout_bwd_reduce_final", "dropout_bwd_apply",
+    "crf_fwd",           "crf_bwd",            "crf_softmax",
 };
 
 struct Record {

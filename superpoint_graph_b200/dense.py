@@ -134,9 +134,14 @@ def _w2d(w):
     return w.view(w.shape[0], w.shape[1]) if w.dim() == 3 else w
 
 
-def chain_forward(inp, M, specs, params, training, saved=None):
+def chain_forward(inp, M, specs, params, training, saved=None, bn_repeats=1):
     """inp: Deferred input.  Returns the Deferred output of the last layer.  If `saved` is a list,
-    per-layer records for chain_backward are appended to it."""
+    per-layer records for chain_backward are appended to it.
+
+    bn_repeats = R: the running statistics of every training-mode BatchNorm take R momentum updates
+    with this batch's statistics, as R evaluations of the chain on the same input would do (ECC_CRFModule
+    runs its filter network once per iteration, ref: learning/modules.py:197).  R updates of momentum m
+    are one update of momentum 1 - (1 - m)^R; num_batches_tracked grows by R."""
     cur = inp
     for sp in specs:
         W = _w2d(params[sp.w])
@@ -154,6 +159,8 @@ def chain_forward(inp, M, specs, params, training, saved=None):
                 if bn.momentum is None:
                     raise NotImplementedError("BatchNorm momentum=None (cumulative average)")
                 mom = bn.momentum
+                if bn_repeats != 1:
+                    mom = 1.0 - (1.0 - mom) ** bn_repeats
             fold = (params[sp.gamma] if sp.gamma is not None else None,
                     params[sp.beta] if sp.beta is not None else None, bn.eps, rm, rv, nbt, mom)
         kpad = _padded_k(sp.cin, cur.ld)
@@ -172,6 +179,8 @@ def chain_forward(inp, M, specs, params, training, saved=None):
             beta = params[sp.beta] if sp.beta is not None else None
             if batch_stats:
                 y, mean, var, scale, shift = res  # statistics + fold come out of the GEMM's merge
+                if bn_repeats != 1 and fold[5] is not None:
+                    fold[5].add_(bn_repeats - 1)  # the merge counted one batch
             else:
                 mean, var = bn.running_mean, bn.running_var
                 scale, shift = ops.bn_fold(mean, var, gamma, beta, bn.eps)

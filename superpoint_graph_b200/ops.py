@@ -228,6 +228,47 @@ def ecc_bwd_x(w, g_out, graph, c_in, add0=None, add1=None):
     return gx
 
 
+# -------------------------------------------------------------------------- ECC-CRF
+CRF_MAX_C = 32  # widest class count the CRF kernels serve (filters [E, C, C])
+
+
+def _crf_graph(graph, n, device):
+    if graph.idxe_host is not None or graph.n_in != n or graph.n_out != n:
+        raise ValueError("the CRF kernels need a square graph of %d nodes without idxe" % n)
+    return graph.to(device)
+
+
+def crf_softmax(x, g=None, out=None):
+    """softmax(x) over rows, or (g given, x a softmax output) its backward x * (g - <g, x>)."""
+    _need_cuda(x, g)
+    x = _c(x)
+    n, C = x.shape
+    if out is None:
+        out = torch.empty_like(x)
+    _lib.call("spg_crf_softmax", x, None if g is None else _c(g), out, n, C, _lib.current_stream())
+    return out
+
+
+def crf_fwd_step(u, q_prev, w, graph, out, softmax):
+    """out = softmax(Z) if softmax else Z, Z = u - ECC(q_prev, w) (matrix filters w [E, C, C])."""
+    _need_cuda(u, q_prev, w, out)
+    n, C = u.shape
+    g = _crf_graph(graph, n, u.device)
+    _lib.call("spg_crf_fwd_step", u, q_prev, w, g["tgt_rowptr"], g["idxn"], out, n, graph.n_edges, C,
+              int(softmax), _lib.current_stream())
+    return out
+
+
+def crf_bwd_step(w, gp, q_prev, du_in, du_out, gp_out, graph):
+    """From gp = dL/dP_r: du_out = du_in + dL/dZ_{r-1}; gp_out (if given) = dL/dP_{r-1} = -dL/dZ_{r-1}."""
+    _need_cuda(w, gp, q_prev, du_in, du_out, gp_out)
+    n, C = q_prev.shape
+    g = _crf_graph(graph, n, w.device)
+    _lib.call("spg_crf_bwd_step", w, gp, q_prev, du_in, du_out, gp_out, g["tgt_rowptr"], g["src_rowptr"],
+              g["src_perm"], g["edge_tgt"], n, graph.n_edges, C, _lib.current_stream())
+    return du_out
+
+
 # ------------------------------------------------------------------------------ GRU
 def gru_fwd(x, h, w_ih, w_hh, b_ih, b_hh, w_ig, b_ig, flags, out=None):
     _need_cuda(x, h, w_ih, w_hh)
