@@ -185,6 +185,50 @@ int spg_rnn_vv_bwd(const float* hs, const float* inps, const float* w, const flo
                    float* dpre, int64_t n_nodes, int hidden, int n_repeats, int flags,
                    void* barrier_ws, spg_stream_t stream);
 
+/* ----------------------------------------------------------- LSTMCellEx   */
+/* (hy, cy) = LSTMCellEx(x, (h, c)).  input_size == hidden_size == H (as built by
+ * learning/graphnet.py:74).  weight_ih/weight_hh [4H,H], bias_* [4H] (added inside the linears,
+ * before the norm), ig_weight [H,H], ig_bias [H]; gates (i, f, g, o) in that order.  flags are the
+ * SPG_GRU_LAYERNORM/INGATE/BIAS bits above: they mean the same for both cells.  H <= 73: the
+ * weights ((2*4+1)*H*H floats) and one row per warp must fit in shared memory, else SPG_E_UNSUPPORTED.
+ * ref: learning/modules.py:281-308 (LSTMCellEx.forward).                                          */
+int spg_lstm_fwd(const float* x, const float* h, const float* c, const float* weight_ih,
+                 const float* weight_hh, const float* bias_ih, const float* bias_hh,
+                 const float* ig_weight, const float* ig_bias, float* hy, float* cy,
+                 int64_t n_rows, int hidden, int flags, spg_stream_t stream);
+/* Backward of the cell for one step, from grad_hy and grad_cy (NULL = 0; d_c may alias it).
+ * d_x, d_h, d_c are final; the parameter gradients are left as per-row factors for one batched
+ * reduction over all recurrent steps: d_gi, d_gh [n,4H] (grads of the pre-norm gate inputs,
+ * biases included: the bias gradients are their column sums), d_q [n,H] (grad of the input-gate
+ * pre-activation), xprime [n,H] (gated input).
+ * ref: the autograd of learning/modules.py:281-308.                                              */
+int spg_lstm_bwd(const float* x, const float* h, const float* c, const float* grad_hy,
+                 const float* grad_cy, const float* weight_ih, const float* weight_hh,
+                 const float* bias_ih, const float* bias_hh, const float* ig_weight,
+                 const float* ig_bias, float* d_x, float* d_h, float* d_c, float* d_gi,
+                 float* d_gh, float* d_q, float* xprime, int64_t n_rows, int hidden, int flags,
+                 spg_stream_t stream);
+/* The fused recurrence of spg_rnn_vv_fwd/bwd with LSTMCellEx as the cell (same conditions,
+ * spg_rnn_vv_supported).  cs [R+1,n,H]: cs[0] = initial cell state on entry (RNNGraphConvModule
+ * starts from zeros), cs[1..R] written.  The backward takes no gradient for any cs[r] (the cell
+ * state never leaves the module), carries dL/dc in d_c_ws [n,H] (scratch) and leaves the factors
+ * of spg_lstm_bwd stacked over the steps (d_gi,d_gh [R,n,4H]; d_q,xprime [R,n,H]).
+ * ref: learning/modules.py:167-183 (the `_isLSTM` branch: cx = 0, (hx, cx) = cell(input, (hx, cx))). */
+int spg_rnn_vv_lstm_fwd(float* hs, float* cs, float* inps, const float* w,
+                        const int32_t* tgt_rowptr, const int32_t* idxn, const float* weight_ih,
+                        const float* weight_hh, const float* bias_ih, const float* bias_hh,
+                        const float* ig_weight, const float* ig_bias, int64_t n_nodes, int hidden,
+                        int n_repeats, int flags, void* barrier_ws, spg_stream_t stream);
+int spg_rnn_vv_lstm_bwd(const float* hs, const float* cs, const float* inps, const float* w,
+                        const float* grad_top, const float* grad_cat, const int32_t* tgt_rowptr,
+                        const int32_t* src_rowptr, const int32_t* src_perm,
+                        const int32_t* edge_tgt, const float* weight_ih, const float* weight_hh,
+                        const float* bias_ih, const float* bias_hh, const float* ig_weight,
+                        const float* ig_bias, float* grad_inp, float* d_h_ws, float* d_c_ws,
+                        float* grad_h0, float* d_gi, float* d_gh, float* d_q, float* xprime,
+                        int64_t n_nodes, int hidden, int n_repeats, int flags, void* barrier_ws,
+                        spg_stream_t stream);
+
 /* ------------------------------------------------------------- dense      */
 /* C[M,N] = opA(A) * opB(B) (+ bias[N]), fp32, FMA accumulation.
  *   a_kmajor=1: A is [M,K] (ld = lda, K contiguous); 0: A is [K,M] (M contiguous)

@@ -58,6 +58,10 @@ enum KernelId {
     K_CRF_FWD,
     K_CRF_BWD,
     K_CRF_SOFTMAX,
+    K_LSTM_FWD,
+    K_LSTM_BWD,
+    K_RNN_LSTM_FWD,
+    K_RNN_LSTM_BWD,
     K_COUNT
 };
 

@@ -24,6 +24,7 @@ static const char* kKernelNames[K_COUNT] = {
     "dropout_rng_next",  "dropout_fwd",        "dropout_mask",        "dropout_bwd_reduce",
     "dropout_bwd_reduce_final", "dropout_bwd_apply",
     "crf_fwd",           "crf_bwd",            "crf_softmax",
+    "lstm_cell_fwd",     "lstm_cell_bwd",      "rnn_ecc_lstm_fwd",    "rnn_ecc_lstm_bwd",
 };
 
 struct Record {
