@@ -417,6 +417,30 @@ int spg_segmax_bn_bwd(const float* g_pooled, int64_t ldg, const int32_t* argmax,
                       const float* var, float eps, int relu, float* s12, float* dY, int64_t lddy,
                       float* workspace, int64_t B, int L, const int64_t* offsets, const int32_t* row_seg,
                       int64_t rows, int C, spg_stream_t stream);
+/* GroupNorm(groups, C) + [ReLU] + [training-mode dropout] over the segments (B, L, offsets) of point rows
+ * Y [rows, ldy], segments as in spg_segmax_fwd (an FC layer's rows are B segments of L = 1).  The
+ * statistics of (segment b, group g) run over the rows of b and the C/groups columns of g, biased variance:
+ *   forward:  mean[b,g] = mean[b,g,0] + mean[b,g,1] ([B, groups, 2]: a float pair, so that a mean that is
+ *             large against the spread keeps its precision), rstd[b,g] = 1/sqrt(var + eps) ([B, groups]);
+ *             both 0 for an empty segment;
+ *             out[r,c] = drop(f((Y[r,c] - mean)*rstd*gamma[c] + beta[c])), f = relu or identity
+ *   backward: from G = dL/d(out): g = relu'(.)*drop'(G), gh = g*gamma, xhat = (Y - mean)*rstd,
+ *             dY = rstd*(gh - mean(gh) - xhat*mean(gh*xhat)) (means over the segment's group),
+ *             dbg = [d_beta | d_gamma] (2*C floats) = [sum g | sum g*xhat] over all rows;
+ *             workspace >= 2*C*spg_group_norm_partials(B) floats
+ * drop as in spg_affine_act (mask index r*C + c).  gamma and beta are required (affine GroupNorm); C <= 1024.
+ * Deterministic: fixed-order sums, no atomics.
+ * ref: learning/pointnet.py:32-35,44-47,88-91,104-107 (nn.GroupNorm(1, C) for norm='layer',
+ * nn.GroupNorm(n_group, C) for norm='group').                                                          */
+int64_t spg_group_norm_partials(int64_t B);
+int spg_group_norm_fwd(const float* Y, int64_t ldy, const float* gamma, const float* beta, float eps, int relu,
+                       float* out, int64_t ldo, float* mean, float* rstd, int64_t B, int L,
+                       const int64_t* offsets, int C, int groups, float p, const int64_t* drop_slot,
+                       spg_stream_t stream);
+int spg_group_norm_bwd(const float* G, int64_t ldg, const float* Y, int64_t ldy, const float* mean,
+                       const float* rstd, const float* gamma, const float* beta, int relu, float* dY,
+                       int64_t lddy, float* dbg, float* workspace, int64_t B, int L, const int64_t* offsets,
+                       int C, int groups, float p, const int64_t* drop_slot, spg_stream_t stream);
 /* dT[b,i,j] = sum_l xy[b,i,l] * dXrows[b*L+l, j], i,j in {0,1}; clouds is the raw
  * [B,F,L] input, dXrows has leading dimension ld.                                    */
 int spg_stn_apply_bwd(const float* clouds, const float* dXrows, int64_t ld, float* dT, int64_t B,

@@ -62,6 +62,9 @@ enum KernelId {
     K_LSTM_BWD,
     K_RNN_LSTM_FWD,
     K_RNN_LSTM_BWD,
+    K_GN_FWD,
+    K_GN_BWD,
+    K_GN_BWD_FINAL,
     K_COUNT
 };
 

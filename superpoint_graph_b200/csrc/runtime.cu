@@ -25,6 +25,7 @@ static const char* kKernelNames[K_COUNT] = {
     "dropout_bwd_reduce_final", "dropout_bwd_apply",
     "crf_fwd",           "crf_bwd",            "crf_softmax",
     "lstm_cell_fwd",     "lstm_cell_bwd",      "rnn_ecc_lstm_fwd",    "rnn_ecc_lstm_bwd",
+    "gn_fwd",            "gn_bwd",             "gn_bwd_final",
 };
 
 struct Record {

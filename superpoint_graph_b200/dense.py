@@ -1,4 +1,4 @@
-"""Chains of (Linear | Conv1d k=1) [+ BatchNorm1d] [+ ReLU] layers with hand-written forward AND
+"""Chains of (Linear | Conv1d k=1) [+ BatchNorm1d | GroupNorm] [+ ReLU] layers with hand-written forward AND
 backward over the C-ABI kernels.
 
 Only the raw (pre-norm) output of each layer is stored; "BatchNorm apply + ReLU" of a layer is
@@ -8,7 +8,10 @@ segmented max-pool, or an explicit materialisation at the end of a chain).
 Reference semantics: the nn.Sequential stacks built by learning/pointnet.py:27-53,83-118 and
 learning/graphnet.py:17-34 (`create_fnet`), in training mode (batch statistics, running-stat
 update with momentum, biased variance for normalisation / unbiased for the running estimate) and
-in eval mode (running statistics).
+in eval mode (running statistics).  A GroupNorm layer (learning/pointnet.py:32-35,44-47,88-91,104-107,
+norm='layer' | 'group') normalises every (segment, group) of its rows; it keeps no running statistics, so
+training and eval compute the same thing.  Its activation is not deferred: ops.group_norm_fwd writes it
+once, and the consumer reads it as is.
 """
 import torch
 import torch.nn as nn
@@ -19,17 +22,19 @@ from . import ops
 class LayerSpec(object):
     """One parametric layer: names index into the flat parameter list given to the chain."""
 
-    __slots__ = ("w", "b", "gamma", "beta", "bn", "relu", "cin", "cout", "drop")
+    __slots__ = ("w", "b", "gamma", "beta", "bn", "relu", "cin", "cout", "drop", "gn")
 
-    def __init__(self, w, b, gamma, beta, bn, relu, cin, cout, drop=0.0):
+    def __init__(self, w, b, gamma, beta, bn, relu, cin, cout, drop=0.0, gn=None):
         self.w, self.b, self.gamma, self.beta = w, b, gamma, beta
         self.bn, self.relu, self.cin, self.cout = bn, relu, cin, cout
         self.drop = drop  # training-mode dropout probability applied after [BatchNorm][ReLU] (0: none)
+        self.gn = gn  # the affine nn.GroupNorm after the layer (then bn is None), or None
 
 
 def parse_sequential(seq, training, params=None):
     """nn.Sequential -> ([LayerSpec], [parameter tensors]).  LayerSpec.w/b/gamma/beta are
-    positions in the returned parameter list; LayerSpec.bn is the BatchNorm module (buffers).
+    positions in the returned parameter list; LayerSpec.bn is the BatchNorm module (buffers), LayerSpec.gn
+    the GroupNorm module (whose weight and bias are gamma and beta).
     With `params` given, the parameters are appended to that list (and it is returned), so that
     several chains index one flat list.
 
@@ -64,7 +69,7 @@ def parse_sequential(seq, training, params=None):
             b = len(params)
             params.append(m.bias)
         i += 1
-        bn, gamma, beta, relu = None, None, None, False
+        bn, gn, gamma, beta, relu = None, None, None, None, False
         if i < len(mods) and isinstance(mods[i], nn.BatchNorm1d):
             bn = mods[i]
             if bn.affine:
@@ -74,7 +79,15 @@ def parse_sequential(seq, training, params=None):
                 params.append(bn.bias)
             i += 1
         elif i < len(mods) and isinstance(mods[i], nn.GroupNorm):
-            raise NotImplementedError("norm='layer'/'group' PointNets are not on the fused path")
+            gn = mods[i]
+            if not gn.affine:
+                raise NotImplementedError("GroupNorm(affine=False) is not on the fused path (no PointNet of the "
+                                          "reference builds one)")
+            gamma = len(params)
+            params.append(gn.weight)
+            beta = len(params)
+            params.append(gn.bias)
+            i += 1
         if i < len(mods) and isinstance(mods[i], nn.ReLU):
             relu = True
             i += 1
@@ -83,7 +96,7 @@ def parse_sequential(seq, training, params=None):
             if training and mods[i].p > 0:
                 drop = float(mods[i].p)
             i += 1
-        specs.append(LayerSpec(w, b, gamma, beta, bn, relu, cin, cout, drop))
+        specs.append(LayerSpec(w, b, gamma, beta, bn, relu, cin, cout, drop, gn))
     return specs, params
 
 
@@ -134,9 +147,12 @@ def _w2d(w):
     return w.view(w.shape[0], w.shape[1]) if w.dim() == 3 else w
 
 
-def chain_forward(inp, M, specs, params, training, saved=None, bn_repeats=1):
+def chain_forward(inp, M, specs, params, training, saved=None, bn_repeats=1, seg=None):
     """inp: Deferred input.  Returns the Deferred output of the last layer.  If `saved` is a list,
     per-layer records for chain_backward are appended to it.
+
+    seg: the segments of the M rows that a GroupNorm layer normalises over, (B, L, offsets, row_seg) as
+    ops.segmax_fwd takes them (a PointNet conv chain: the clouds); None: every row is its own sample (FC).
 
     bn_repeats = R: the running statistics of every training-mode BatchNorm take R momentum updates
     with this batch's statistics, as R evaluations of the chain on the same input would do (ECC_CRFModule
@@ -184,13 +200,25 @@ def chain_forward(inp, M, specs, params, training, saved=None, bn_repeats=1):
             else:
                 mean, var = bn.running_mean, bn.running_var
                 scale, shift = ops.bn_fold(mean, var, gamma, beta, bn.eps)
-        nxt = act = Deferred(y, sp.cout, sp.cout, scale, shift, sp.relu)
-        if sp.drop > 0 and training:
-            # dropout cannot ride in a GEMM prologue: BatchNorm-apply, ReLU and the mask in one pass, and
-            # the consumer (next layer's GEMM and weight gradient) reads the dropped activation as is
-            nxt.drop = (sp.drop, ops.dropout_slot(y.device))
-            act = Deferred(ops.affine_act(y, sp.cout, M, sp.cout, scale, shift, sp.relu, drop=nxt.drop),
-                           sp.cout, sp.cout)
+        if sp.gn is not None:
+            # GroupNorm, ReLU and dropout in one pass over y; the consumer (next layer's GEMM and weight
+            # gradient, or the max-pool) reads the activation as is.  The record keeps y and the per-(segment,
+            # group) mean and rstd (in the `var` slot) for ops.group_norm_bwd.
+            drop = (sp.drop, ops.dropout_slot(y.device)) if (sp.drop > 0 and training) else None
+            a, mean, var = ops.group_norm_fwd(y, sp.cout, ops.row_segs(M) if seg is None else seg, sp.cout,
+                                              sp.gn.num_groups, params[sp.gamma], params[sp.beta], sp.gn.eps,
+                                              sp.relu, drop=drop)
+            nxt = Deferred(y, sp.cout, sp.cout)
+            nxt.drop = drop
+            act = Deferred(a, sp.cout, sp.cout)
+        else:
+            nxt = act = Deferred(y, sp.cout, sp.cout, scale, shift, sp.relu)
+            if sp.drop > 0 and training:
+                # dropout cannot ride in a GEMM prologue: BatchNorm-apply, ReLU and the mask in one pass, and
+                # the consumer (next layer's GEMM and weight gradient) reads the dropped activation as is
+                nxt.drop = (sp.drop, ops.dropout_slot(y.device))
+                act = Deferred(ops.affine_act(y, sp.cout, M, sp.cout, scale, shift, sp.relu, drop=nxt.drop),
+                               sp.cout, sp.cout)
         if saved is not None:
             saved.append((cur, nxt, mean, var))
         cur = act
@@ -202,11 +230,12 @@ def _accumulate_grad(prm, g):
         prm.grad = g if prm.grad is None else prm.grad + g
 
 
-def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_g=False, pooled=None):
+def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_g=False, pooled=None, seg=None):
     """G: gradient w.r.t. the chain's final *activated* output [M, C_last].
     `grads` (list aligned with params) is filled in place.  Returns the gradient w.r.t. the
     chain input's activated value [M, cin_0] (or None).  If the chain's output was max-pooled over the
-    segments `seg` (ops.segmax_fwd), G is None and pooled = (g_pooled, ldg, argmax, seg).
+    segments `seg` (ops.segmax_fwd), G is None and pooled = (g_pooled, ldg, argmax, seg).  `seg` is the
+    segment description chain_forward had (GroupNorm layers).
 
     Where the data-gradient GEMM of a layer runs on the wgmma kernel, the BatchNorm/ReLU backward
     around it is fused into that ONE launch: the prologue turns dL/d(activation) into dL/dY on the
@@ -217,7 +246,11 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
     A layer with dropout masks the incoming gradient inside its own BatchNorm/ReLU backward
     (act_bwd_reduce / act_bwd_apply with `drop`, the mask regenerated from the forward's slot); both
     fused paths that would read that gradient unmasked are off for it: the lazy prologue of its
-    data-gradient GEMM and the epilogue sums of the GEMM of the layer above."""
+    data-gradient GEMM and the epilogue sums of the GEMM of the layer above.
+
+    A GroupNorm layer's backward is ops.group_norm_bwd (dropout and ReLU masks included); none of the fused
+    BatchNorm paths applies to it, and its bias gradient is a real column sum: a per-channel bias is not
+    removed by a per-group mean."""
     red = None  # s1|s2 of the current layer, if the GEMM that produced G already reduced them
     for li in range(len(specs) - 1, -1, -1):
         sp = specs[li]
@@ -241,6 +274,10 @@ def chain_backward(G, ldg, M, specs, params, saved, need_input_grad, grads, own_
             if sp.gamma is not None:
                 grads[sp.gamma] = s2
                 grads[sp.beta] = s1
+        elif sp.gn is not None:
+            dY, grads[sp.gamma], grads[sp.beta] = ops.group_norm_bwd(
+                G, ldg, nxt.raw, nxt.ld, mean, var, params[sp.gamma], params[sp.beta],
+                ops.row_segs(M) if seg is None else seg, C, sp.gn.num_groups, sp.relu, drop=drop)
         elif sp.bn is not None:
             eps = sp.bn.eps
             assert drop is None or red is None  # the layer above never reduces for a dropout layer (see bnred)

@@ -780,6 +780,43 @@ def segmax_bn_bwd(g_pooled, ldg, argmax, Y, ldy, scale, shift, mean, var, eps, r
     return s12[:C], s12[C:], dY
 
 
+def row_segs(M):
+    """The segment description of M rows that are each their own sample (an FC layer's rows)."""
+    return (M, 1, None, None)
+
+
+def group_norm_fwd(Y, ldy, seg, C, groups, gamma, beta, eps, relu, drop=None, out=None, ldo=None):
+    """GroupNorm(groups, C) of Y [rows, C] over each segment of seg (as segmax_fwd), then ReLU if relu, then
+    dropout with drop = (p, slot) (as affine_act).  Returns (out [rows, C], mean [B, groups, 2], rstd [B, groups]);
+    the mean is a pair of floats (hi, lo) whose sum is the group's mean."""
+    B, L, offsets, _ = seg
+    _need_cuda(Y, gamma, beta, offsets)
+    M = _seg_rows(seg)
+    dev = Y.device
+    if out is None:
+        out = torch.empty((M, C), dtype=torch.float32, device=dev)
+        ldo = C
+    mean = torch.empty((B, groups, 2), dtype=torch.float32, device=dev)
+    rstd = torch.empty((B, groups), dtype=torch.float32, device=dev)
+    _lib.call("spg_group_norm_fwd", Y, ldy, _c(gamma), _c(beta), float(eps), int(bool(relu)), out, ldo, mean, rstd,
+              B, L, offsets, C, groups, *_drop(drop), _lib.current_stream())
+    return out, mean, rstd
+
+
+def group_norm_bwd(G, ldg, Y, ldy, mean, rstd, gamma, beta, seg, C, groups, relu, drop=None):
+    """Backward of group_norm_fwd from G = dL/d(out): returns (dY [rows, C], d_gamma [C], d_beta [C])."""
+    B, L, offsets, _ = seg
+    _need_cuda(G, Y, gamma, beta, offsets)
+    M = _seg_rows(seg)
+    dev = G.device
+    dY = torch.empty((M, C), dtype=torch.float32, device=dev)
+    dbg = torch.empty(2 * C, dtype=torch.float32, device=dev)
+    ws = workspace(2 * C * int(_lib.lib().spg_group_norm_partials(int(B))), dev)
+    _lib.call("spg_group_norm_bwd", G, ldg, Y, ldy, mean, rstd, _c(gamma), _c(beta), int(bool(relu)), dY, C, dbg,
+              ws, B, L, offsets, C, groups, *_drop(drop), _lib.current_stream())
+    return dY, dbg[C:], dbg[:C]
+
+
 def stn_apply_bwd(clouds, dXrows, ld):
     _need_cuda(clouds, dXrows)
     clouds = _c(clouds)

@@ -95,7 +95,7 @@ class _Layout(object):
         saved, argmax = record
         # chain_backward fuses the pool backward into the last layer's BatchNorm backward
         return chain_backward(None, specs[-1].cout, self.M, specs, params, saved, need_input_grad, grads,
-                              pooled=(g_pool, g_pool.shape[1], argmax, self.seg))
+                              pooled=(g_pool, g_pool.shape[1], argmax, self.seg), seg=self.seg)
 
 
 class _Clouds(_Layout):
@@ -183,13 +183,14 @@ def _conv_layers(specs, params):
 
 def _pool(layout, T, specs, params, training, fused, pooled):
     """Point-wise chain `specs` over the layout's point rows (xy-transformed by T + I if T is given),
-    max-pooled per cloud into pooled[:, :C].  Returns what its backward needs, (layer records, argmax),
+    max-pooled per cloud into pooled[:, :C]; a GroupNorm layer of the chain normalises over each cloud.  Returns what its backward needs, (layer records, argmax),
     in training mode."""
     if fused:
         layout.fused_pool(specs, params, T, pooled)
         return None
     sv = [] if training else None
-    out = chain_forward(Deferred(layout.rows(T), layout.ld, specs[0].cin), layout.M, specs, params, training, sv)
+    out = chain_forward(Deferred(layout.rows(T), layout.ld, specs[0].cin), layout.M, specs, params, training, sv,
+                        seg=layout.seg)
     argmax = layout.segmax(out, pooled)
     return (sv, argmax) if training else None
 
