@@ -585,6 +585,88 @@ int spg_nn1_interpolate(const float* xyz_ref, int64_t n_ref, const float* xyz_qu
                         const int64_t* labels_ref, int64_t* labels_out, int32_t* nn_index_out,
                         spg_stream_t stream);
 
+/* ------------------------------------------- learned partition (supervized_partition/losses.py)
+ * Edge arrays src/tgt are int64 [E] device arrays; is_transition is uint8 [E] (0 = intra, 1 = inter);
+ * pred_in_component int64 [V].  Endpoints outside [0, V) are skipped (never read).  No float atomics:
+ * every float output is bit-reproducible.
+ * spg_lp_sort_workspace: bytes of the CUB scratch (`workspace`) of every sorting/scanning call below
+ * for up to n items (2E for spg_lp_incidence, max(V, E) for spg_lp_xpart, V for spg_lp_seal).        */
+int spg_lp_sort_workspace(int64_t n, int64_t* bytes);
+/* Per-vertex incidence CSR of the edge endpoints: entry j < E is the source side of edge j, j >= E the
+ * target side of edge j - E; rowptr [V+1], entry [2E] sorted by vertex, stably (by j within a vertex).
+ * keys_tmp, keys_sorted, vals_tmp: int32 [2E] scratch.  No reference counterpart: the gather CSR of the
+ * deterministic backward of compute_dist (ref: supervized_partition/losses.py:31-42 under autograd).  */
+int spg_lp_incidence(const int64_t* src, const int64_t* tgt, int64_t n_ver, int64_t n_edges, int32_t* rowptr,
+                     int32_t* entry, int32_t* keys_tmp, int32_t* keys_sorted, int32_t* vals_tmp, void* workspace,
+                     int64_t workspace_bytes, spg_stream_t stream);
+/* diff[e] from embeddings emb [V, D] (dist_type 0 = euclidian: |x_s - x_t|^2, 1 = intrinsic:
+ * (acos(0.999 x_s.x_t) - acos(0.999)) / (acos(-0.999) - acos(0.999)) * 3.141592, 2 = scalar: x_s.x_t - 1),
+ * fp64 inside; coef [E] (intrinsic, scalar; may be NULL for euclidian) = d diff / d (x_s.x_t).
+ * Backward: gemb [V, D] = dL/demb from gdiff [E], gathered through the incidence CSR.
+ * ref: supervized_partition/losses.py:31-42                                                              */
+int spg_lp_dist_fwd(const float* emb, int64_t n_ver, int D, const int64_t* src, const int64_t* tgt, int64_t n_edges,
+                    int dist_type, float* diff, float* coef, spg_stream_t stream);
+int spg_lp_dist_bwd(const float* emb, int64_t n_ver, int D, const int64_t* src, const int64_t* tgt, int64_t n_edges,
+                    int dist_type, const float* coef, const float* gdiff, const int32_t* rowptr, const int32_t* entry,
+                    float* gemb, spg_stream_t stream);
+/* compute_loss: loss [2] = (sum over is_transition == 0 of the intra term, sum over is_transition == 1 of
+ * the inter term), fp64 sums over spg_lp_loss_partials() fixed blocks (partials: 2 doubles per block),
+ * merged in a fixed order.  intra: 0 = tv w*sqrt(d+1e-10), 1 = laplacian w*d, 2 = TVH
+ * 0.2*w*(sqrt(1+d/0.04)-1); inter: 0 = zhang clamp(w*(beta - sqrt(d+1e-10)), min=0) (beta = 1.0471975512 for
+ * dist_type 1, else 1), 1 = TVminus w*sqrt(d+1e-10), -1 = none (loss[1] = 0).
+ * Backward: gdiff [E] from gloss [2] (device).  ref: supervized_partition/losses.py:24-29,44-64          */
+int64_t spg_lp_loss_partials(void);
+int spg_lp_loss_fwd(const float* diff, const float* weights, const uint8_t* is_transition, int64_t n_edges,
+                    int intra, int inter, int dist_type, double* partials, float* loss, spg_stream_t stream);
+int spg_lp_loss_bwd(const float* diff, const float* weights, const uint8_t* is_transition, int64_t n_edges,
+                    int intra, int inter, int dist_type, const float* gloss, float* gdiff, spg_stream_t stream);
+/* crosspartition weights: connected components of the edges with is_transition == 0 and
+ * pred_in_component[s] == pred_in_component[t] (components numbered by their smallest vertex:
+ * in_component_x [V], comp_size [V] (first n_comp used), n_comp [1]); every transition edge between
+ * components (c1, c2) gets 1 + min(|c1|, |c2|) / #(transition edges between c1 and c2) * transition_factor
+ * (fp64, rounded once), every other edge 1.  Scratch: parent, is_root, root_rank int32 [V];
+ * keys_tmp, keys_sorted uint64 [E]; vals_tmp, vals_sorted int32 [E].
+ * ref: supervized_partition/losses.py:130-158 (+ partition/ply_c/connected_components.cpp:17-110, cutoff 0) */
+int spg_lp_xpart(const int64_t* src, const int64_t* tgt, const uint8_t* is_transition,
+                 const int64_t* pred_in_component, int64_t n_ver, int64_t n_edges, double transition_factor,
+                 float* weights, int32_t* in_component_x, int32_t* comp_size, int32_t* n_comp, int32_t* parent,
+                 int32_t* is_root, int32_t* root_rank, uint64_t* keys_tmp, uint64_t* keys_sorted, int32_t* vals_tmp,
+                 int32_t* vals_sorted, void* workspace, int64_t workspace_bytes, spg_stream_t stream);
+/* SEAL weights: w[c] = |c| - (frequency of the most common object id in c) for the n_comp predicted
+ * components (objects: int64 [V], 0 <= id < 2^32); transition edges get 1 + max(w[c_s], w[c_t]) *
+ * transition_factor (fp64, rounded once), others 1; w_per_component [n_comp] (may be NULL).
+ * Scratch: size_tmp, maxfreq_tmp int32 [n_comp]; keys_tmp, keys_sorted uint64 [V].
+ * ref: supervized_partition/losses.py:119-128,168-173                                                    */
+int spg_lp_seal(const int64_t* src, const int64_t* tgt, const uint8_t* is_transition, const int64_t* pred_in_component,
+                const int64_t* objects, int64_t n_ver, int64_t n_edges, int64_t n_comp, double transition_factor,
+                float* weights, int32_t* w_per_component, int32_t* size_tmp, int32_t* maxfreq_tmp, uint64_t* keys_tmp,
+                uint64_t* keys_sorted, void* workspace, int64_t workspace_bytes, spg_stream_t stream);
+/* weights[e] = is_transition[e] != 0 ? w_transition : w_other ('none', 'proportional';
+ * ref: supervized_partition/losses.py:96-101)                                                            */
+int spg_lp_fill_weights(const uint8_t* is_transition, int64_t n_edges, float w_other, float w_transition,
+                        float* weights, spg_stream_t stream);
+/* counts [2] (int64, device) = (#(truth != 0 and pred != 0), #(truth != 0)); pred may be NULL (counts[0] = 0).
+ * For 0/1 masks these are the numerator and denominator of compute_boundary_recall(truth, pred) and, with
+ * the arguments swapped, of compute_boundary_precision.  ref: learning/metrics.py:87-92                  */
+int spg_lp_count(const uint8_t* truth, const uint8_t* pred, int64_t n, int64_t* counts, spg_stream_t stream);
+/* cut pursuit's edge weights (double [E]): threshold > 0: diff > 1 ? (float)threshold : 1; threshold < 0:
+ * expf(diff * (float)threshold) / exp(threshold); 0: 1.  ref: supervized_partition/losses.py:68-72        */
+int spg_lp_edge_weight(const float* diff, int64_t n_edges, double threshold, double* edge_weight,
+                       spg_stream_t stream);
+/* relax_edge_binary in place on relaxed [E] (uint8 0/1), `tolerance` rounds of: mark the endpoints of the
+ * set edges (vertex_mark uint8 [V]); set edge 0 if some edge's source is unmarked and edge 1 if some edge's
+ * source is marked (losses.py:184 indexes with the mark values); set every edge whose target is marked.
+ * hit: int32 scratch; status [1] = 1 if edge 1 was needed but E == 1 (numpy raises IndexError).
+ * ref: supervized_partition/losses.py:175-186                                                            */
+int spg_lp_relax(uint8_t* relaxed, const int64_t* src, const int64_t* tgt, int64_t n_ver, int64_t n_edges,
+                 int tolerance, uint8_t* vertex_mark, int32_t* hit, int32_t* status, spg_stream_t stream);
+/* pred [V] (int64, zeroed here) = for the members (point_ids[comp_ptr[c]:comp_ptr[c+1]]) of every component c
+ * the first argmax over k of the int64 sum of labels[v, 1 + k], k < n_classes (labels int64 [V, ld_labels]).
+ * ref: partition/provider.py:689-695                                                                     */
+int spg_lp_perfect_prediction(const int64_t* comp_ptr, const int64_t* point_ids, int64_t n_comp,
+                              const int64_t* labels, int64_t ld_labels, int n_classes, int64_t n_ver, int64_t* pred,
+                              spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -65,6 +65,17 @@ enum KernelId {
     K_GN_FWD,
     K_GN_BWD,
     K_GN_BWD_FINAL,
+    K_LP_INCIDENCE,
+    K_LP_DIST_FWD,
+    K_LP_DIST_BWD,
+    K_LP_LOSS_FWD,
+    K_LP_LOSS_BWD,
+    K_LP_CC,
+    K_LP_XPART,
+    K_LP_SEAL,
+    K_LP_WEIGHTS,
+    K_LP_RELAX,
+    K_LP_METRICS,
     K_COUNT
 };
 

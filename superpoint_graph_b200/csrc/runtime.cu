@@ -26,6 +26,9 @@ static const char* kKernelNames[K_COUNT] = {
     "crf_fwd",           "crf_bwd",            "crf_softmax",
     "lstm_cell_fwd",     "lstm_cell_bwd",      "rnn_ecc_lstm_fwd",    "rnn_ecc_lstm_bwd",
     "gn_fwd",            "gn_bwd",             "gn_bwd_final",
+    "lp_incidence",      "lp_dist_fwd",        "lp_dist_bwd",         "lp_loss_fwd",
+    "lp_loss_bwd",       "lp_cc",              "lp_xpart",            "lp_seal",
+    "lp_weights",        "lp_relax",           "lp_metrics",
 };
 
 struct Record {

@@ -1133,3 +1133,150 @@ def pointnet_fused_eval(clouds, T, image, bias, widths, pooled, ldp):
 
 
 FUSED_FLOPS = [0]  # algorithmic FLOPs through the fused eval trunk; read by bench.py
+
+
+# ------------------------------------------------------------------ learned partition (csrc/partition.cu)
+LP_DIST = {"euclidian": 0, "intrinsic": 1, "scalar": 2}
+LP_INTRA = {"tv": 0, "laplacian": 1, "TVH": 2}
+LP_INTER = {None: -1, "zhang": 0, "TVminus": 1}
+
+
+def _lp_sort_ws(n, dev):
+    nbytes = torch.zeros(1, dtype=torch.int64)
+    _lib.call("spg_lp_sort_workspace", int(n), nbytes)
+    ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=dev)
+    return ws, ws.numel()
+
+
+def lp_incidence(src, tgt, n_ver):
+    """Per-vertex CSR of the edge endpoints: (rowptr int32 [V+1], entry int32 [2E]); entry j < E is the source
+    side of edge j, j >= E the target side of edge j - E."""
+    _need_cuda(src, tgt)
+    dev, E = src.device, src.numel()
+    i32 = dict(dtype=torch.int32, device=dev)
+    rowptr, entry = torch.empty(n_ver + 1, **i32), torch.empty(2 * E, **i32)
+    k0, k1, v0 = torch.empty(2 * E, **i32), torch.empty(2 * E, **i32), torch.empty(2 * E, **i32)
+    ws, nb = _lp_sort_ws(2 * E, dev)
+    _lib.call("spg_lp_incidence", src, tgt, n_ver, E, rowptr, entry, k0, k1, v0, ws, nb, _lib.current_stream())
+    return rowptr, entry
+
+
+def lp_dist_fwd(emb, src, tgt, dist_type):
+    """(diff [E], coef [E] or None): compute_dist and the factor d diff / d <x_s, x_t> of its backward."""
+    _need_cuda(emb, src, tgt)
+    assert emb.dtype == torch.float32 and emb.dim() == 2 and emb.is_contiguous()
+    assert src.dtype == torch.int64 and tgt.dtype == torch.int64
+    E, dev = src.numel(), emb.device
+    dt = LP_DIST[dist_type]
+    diff = torch.empty(E, dtype=torch.float32, device=dev)
+    coef = None if dt == 0 else torch.empty(E, dtype=torch.float32, device=dev)
+    _lib.call("spg_lp_dist_fwd", emb, emb.shape[0], emb.shape[1], src, tgt, E, dt, diff, coef, _lib.current_stream())
+    return diff, coef
+
+
+def lp_dist_bwd(emb, src, tgt, dist_type, coef, gdiff, incidence):
+    _need_cuda(emb, src, tgt, coef, gdiff)
+    rowptr, entry = incidence
+    gemb = torch.empty_like(emb)
+    _lib.call("spg_lp_dist_bwd", emb, emb.shape[0], emb.shape[1], src, tgt, src.numel(), LP_DIST[dist_type], coef,
+              _c(gdiff), rowptr, entry, gemb, _lib.current_stream())
+    return gemb
+
+
+def lp_loss_fwd(diff, weights, is_transition, intra, inter, dist_type):
+    """float32 [2] = (loss1, loss2) of compute_loss; is_transition uint8."""
+    _need_cuda(diff, weights, is_transition)
+    assert diff.dtype == torch.float32 and weights.dtype == torch.float32 and is_transition.dtype == torch.uint8
+    dev = diff.device
+    part = torch.empty(2 * int(_lib.lib().spg_lp_loss_partials()), dtype=torch.float64, device=dev)
+    loss = torch.empty(2, dtype=torch.float32, device=dev)
+    _lib.call("spg_lp_loss_fwd", _c(diff), _c(weights), _c(is_transition), diff.numel(), LP_INTRA[intra],
+              LP_INTER[inter], LP_DIST[dist_type], part, loss, _lib.current_stream())
+    return loss
+
+
+def lp_loss_bwd(diff, weights, is_transition, intra, inter, dist_type, gloss):
+    _need_cuda(diff, weights, is_transition, gloss)
+    gdiff = torch.empty_like(diff)
+    _lib.call("spg_lp_loss_bwd", _c(diff), _c(weights), _c(is_transition), diff.numel(), LP_INTRA[intra],
+              LP_INTER[inter], LP_DIST[dist_type], _c(gloss), gdiff, _lib.current_stream())
+    return gdiff
+
+
+def lp_xpart(src, tgt, is_transition, pred_in_component, n_ver, transition_factor):
+    """crosspartition weights: (weights float32 [E], in_component_x int32 [V], comp_size int32 [V] (the first
+    n_comp are used), n_comp int32 [1]), all on the device."""
+    _need_cuda(src, tgt, is_transition, pred_in_component)
+    dev, E = src.device, src.numel()
+    i32 = dict(dtype=torch.int32, device=dev)
+    w = torch.empty(E, dtype=torch.float32, device=dev)
+    inx, size, ncomp = torch.empty(n_ver, **i32), torch.empty(n_ver, **i32), torch.empty(1, **i32)
+    par, root, rank = torch.empty(n_ver, **i32), torch.empty(n_ver, **i32), torch.empty(n_ver, **i32)
+    k0 = torch.empty(E, dtype=torch.int64, device=dev)
+    k1 = torch.empty(E, dtype=torch.int64, device=dev)
+    v0, v1 = torch.empty(E, **i32), torch.empty(E, **i32)
+    ws, nb = _lp_sort_ws(max(n_ver, E), dev)
+    _lib.call("spg_lp_xpart", src, tgt, is_transition, pred_in_component, n_ver, E, float(transition_factor), w, inx,
+              size, ncomp, par, root, rank, k0, k1, v0, v1, ws, nb, _lib.current_stream())
+    return w, inx, size, ncomp
+
+
+def lp_seal(src, tgt, is_transition, pred_in_component, objects, n_comp, transition_factor):
+    """SEAL weights: (weights float32 [E], w_per_component int32 [n_comp])."""
+    _need_cuda(src, tgt, is_transition, pred_in_component, objects)
+    dev, E, V = src.device, src.numel(), pred_in_component.numel()
+    i32 = dict(dtype=torch.int32, device=dev)
+    w, wc = torch.empty(E, dtype=torch.float32, device=dev), torch.empty(n_comp, **i32)
+    st, mt = torch.empty(n_comp, **i32), torch.empty(n_comp, **i32)
+    k0, k1 = torch.empty(V, dtype=torch.int64, device=dev), torch.empty(V, dtype=torch.int64, device=dev)
+    ws, nb = _lp_sort_ws(V, dev)
+    _lib.call("spg_lp_seal", src, tgt, is_transition, pred_in_component, objects, V, E, n_comp,
+              float(transition_factor), w, wc, st, mt, k0, k1, ws, nb, _lib.current_stream())
+    return w, wc
+
+
+def lp_fill_weights(is_transition, w_other, w_transition):
+    _need_cuda(is_transition)
+    w = torch.empty(is_transition.numel(), dtype=torch.float32, device=is_transition.device)
+    _lib.call("spg_lp_fill_weights", is_transition, is_transition.numel(), float(w_other), float(w_transition), w,
+              _lib.current_stream())
+    return w
+
+
+def lp_count(truth, pred=None):
+    """int64 [2] on the device: (#(truth and pred), #truth) of uint8 masks."""
+    _need_cuda(truth, pred)
+    counts = torch.empty(2, dtype=torch.int64, device=truth.device)
+    _lib.call("spg_lp_count", _c(truth), None if pred is None else _c(pred), truth.numel(), counts,
+              _lib.current_stream())
+    return counts
+
+
+def lp_edge_weight(diff, threshold):
+    _need_cuda(diff)
+    out = torch.empty(diff.numel(), dtype=torch.float64, device=diff.device)
+    _lib.call("spg_lp_edge_weight", _c(diff), diff.numel(), float(threshold), out, _lib.current_stream())
+    return out
+
+
+def lp_relax(relaxed, src, tgt, n_ver, tolerance):
+    """relax_edge_binary in place on the uint8 mask `relaxed`; returns the status word (1: numpy's IndexError)."""
+    _need_cuda(relaxed, src, tgt)
+    assert relaxed.dtype == torch.uint8 and relaxed.is_contiguous()
+    dev = relaxed.device
+    mark = torch.empty(max(n_ver, 1), dtype=torch.uint8, device=dev)
+    hit, status = torch.empty(1, dtype=torch.int32, device=dev), torch.empty(1, dtype=torch.int32, device=dev)
+    _lib.call("spg_lp_relax", relaxed, src, tgt, n_ver, relaxed.numel(), int(tolerance), mark, hit, status,
+              _lib.current_stream())
+    return status
+
+
+def lp_perfect_prediction(comp_ptr, point_ids, labels, n_ver):
+    """int64 [n_ver]: the first majority label of each point's component (labels int64 [V, 1 + C])."""
+    _need_cuda(comp_ptr, point_ids, labels)
+    assert labels.dtype == torch.int64 and labels.dim() == 2
+    labels = _c(labels)
+    pred = torch.empty(n_ver, dtype=torch.int64, device=labels.device)
+    _lib.call("spg_lp_perfect_prediction", comp_ptr, point_ids, comp_ptr.numel() - 1, labels, labels.shape[1],
+              labels.shape[1] - 1, n_ver, pred, _lib.current_stream())
+    return pred
