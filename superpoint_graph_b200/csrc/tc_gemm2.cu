@@ -18,8 +18,13 @@
 //                 STATS : batch statistics of C (pivoted sums kept per warp across tiles)
 //                 BNRED : BatchNorm-backward sums of the layer BELOW (C is its dL/d(act)):
 //                         s1 = sum gz, s2 = sum gz*xhat with gz = relu'(y2) * C
+//               The two warpgroups take turns (ping-pong, two named barriers): warpgroup 1 issues a tile's
+//               MMAs once warpgroup 0 has issued its own for that tile, warpgroup 0 those of the next tile
+//               once warpgroup 1 is done, so each one's epilogue runs under the other's MMAs.
 //   warps 8-15  producers: coalesced 128-bit loads of A (next chunks prefetched in registers), fused
-//               prologue, tf32 hi/lo split, SWIZZLE_128B K-major tiles, 2..4-stage ring
+//               prologue, tf32 hi/lo split, SWIZZLE_128B K-major tiles.  Producer warpgroup p fills
+//               the 64-row half p of every tile into its own 2..4-stage ring, read by consumer warpgroup
+//               p alone: a warpgroup in its epilogue holds back none of the other one's stages.
 //                 AFFINE : f = relu(a*scale + shift)          (forward: BN apply + ReLU)
 //                 BNBWD  : f = scale*(gz - s1/M - xhat*s2/M)  (backward: A = dL/d(act),
 //                          A2 = raw output y of the layer; optional side store of f)
@@ -46,7 +51,9 @@ constexpr int T2_MAX_STAGES = 4;  // the A ring gets as many stages as fit next 
 constexpr int T2_EPI_WARPS = 8, T2_PROD_WARPS = 8;  // consumers: two warpgroups of 64 rows each
 constexpr int T2_THREADS = (T2_EPI_WARPS + T2_PROD_WARPS) * 32;  // 512
 constexpr int T2_A_BYTES = T2_BM * T2_KC * 4;                    // 16 KB (hi or lo)
-constexpr int T2_STAGE_BYTES = 2 * T2_A_BYTES;
+constexpr int T2_STAGE_BYTES = 2 * T2_A_BYTES;                   // one stage of both rings
+constexpr int T2_HALF_A_BYTES = T2_A_BYTES / 2;                  // 64 rows: one warpgroup's hi or lo
+constexpr int T2_HALF_STAGE_BYTES = 2 * T2_HALF_A_BYTES;         // one stage of one warpgroup's ring
 
 enum { PRO_AFFINE = 0, PRO_BNBWD = 1 };
 enum { EPI_NONE = 0, EPI_STATS = 1, EPI_BNRED = 2 };
@@ -82,6 +89,51 @@ struct Tc2Args {
     int nstages;   // A-ring depth (2..4)
 };
 
+// Named barriers 1 and 2 order the consumer warpgroups' MMA phases (0 is __syncthreads)
+constexpr int T2_TURN_BAR = 1;
+constexpr int T2_TURN_THREADS = 2 * 128;
+__device__ __forceinline__ void turn_wait(int id) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(T2_TURN_THREADS) : "memory");
+}
+__device__ __forceinline__ void turn_pass(int id) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(T2_TURN_THREADS) : "memory");
+}
+
+// Predicated global stores that the compiler may not take for writes to shared memory (C and the dY side
+// store: nothing in the kernel reads them back, so column sums in shared memory need no reload after them)
+__device__ __forceinline__ void st_global2(float* ptr, float2 v, bool pred) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p st.global.v2.f32 [%0], {%1, %2};\n\t}" ::"l"(ptr),
+        "f"(v.x), "f"(v.y), "r"((int)pred));
+}
+__device__ __forceinline__ void st_global4(float* ptr, float4 v, bool pred) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t@p st.global.v4.f32 [%0], {%1, %2, %3, %4};\n\t}" ::"l"(ptr),
+        "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "r"((int)pred));
+}
+
+// Column sums of a block of 4 columns over the 8 lanes that hold them (the lanes with the same lane % 4; lane
+// r = lane / 4 holds rows r and r + 8): v[2k], v[2k + 1] are this lane's two partial sums of block column k.
+// Reduce-scatter in three halving steps over lane distance 4, 8 and 16.  Every sum is formed from the same
+// pairs, in the same order, as a butterfly (x += shfl_xor(x, 4), 8, 16) on each value forms it, so it is
+// bitwise what that butterfly leaves in every lane.  Lane r gets sum v[4(r & 1) + 2((r >> 1) & 1) + (r >> 2)].
+__device__ __forceinline__ float reduce_scatter8(const float (&v)[8], int r) {
+    const bool b0 = r & 1, b1 = r & 2, b2 = r & 4;
+    float w[4], x[2];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float keep = b0 ? v[i + 4] : v[i], send = b0 ? v[i] : v[i + 4];
+        w[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const float keep = b1 ? w[i + 2] : w[i], send = b1 ? w[i] : w[i + 2];
+        x[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+    }
+    const float keep = b2 ? x[1] : x[0], send = b2 ? x[0] : x[1];
+    return keep + __shfl_xor_sync(0xffffffffu, send, 16);
+}
+
 // 2-D TMA load global -> shared, completion counted on an mbarrier (coordinates: {x = innermost, y})
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
     asm volatile(
@@ -98,7 +150,7 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     // it): SWIZZLE_128B atoms need that, and no spare bytes are reserved for a manual round-up
     uint8_t* smem = smem_raw;
     if ((smem_u32(smem_raw) & 1023u) != 0u) __trap();
-    __shared__ __align__(8) uint64_t bars[2 * T2_MAX_STAGES + 1];
+    __shared__ __align__(8) uint64_t bars[4 * T2_MAX_STAGES + 1];
 
     const int t = threadIdx.x;
     const int warp = t >> 5, lane = t & 31;
@@ -106,19 +158,23 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     const int n0 = blockIdx.y * NS;  // first output channel of this CTA's slice
     const int64_t tiles = (p.M + T2_BM - 1) / T2_BM;
     const int nst = p.nstages;
+    // two A rings, one per 64-row half of the tile: ring h = nst stages of [hi|lo][64 rows][128 B]
+    auto ring = [&](int h) { return smem_u32(smem) + (uint32_t)(h * nst) * T2_HALF_STAGE_BYTES; };
     uint8_t* wres = smem + (size_t)nst * T2_STAGE_BYTES;  // resident weights: [nk][hi|lo][NS][128 B]
 
     const uint32_t bars_u32 = smem_u32(&bars[0]);
-    auto bar_full = [&](int s) { return bars_u32 + 8u * (uint32_t)s; };
-    auto bar_empty = [&](int s) { return bars_u32 + 8u * (uint32_t)(T2_MAX_STAGES + s); };
-    const uint32_t bar_w = bars_u32 + 8u * (2 * T2_MAX_STAGES);
+    auto bar_full = [&](int h, int s) { return bars_u32 + 8u * (uint32_t)(h * T2_MAX_STAGES + s); };
+    auto bar_empty = [&](int h, int s) { return bars_u32 + 8u * (uint32_t)((2 + h) * T2_MAX_STAGES + s); };
+    const uint32_t bar_w = bars_u32 + 8u * (4 * T2_MAX_STAGES);
 
     if (t == 0) {
 #pragma unroll
-        for (int s = 0; s < T2_MAX_STAGES; ++s) {
-            mbar_init(bar_full(s), T2_PROD_WARPS);  // one elected arrival per producer warp
-            mbar_init(bar_empty(s), T2_EPI_WARPS);  // one elected arrival per consumer warp
-        }
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int s = 0; s < T2_MAX_STAGES; ++s) {
+                mbar_init(bar_full(h, s), T2_PROD_WARPS / 2);  // one elected arrival per producer warp of h
+                mbar_init(bar_empty(h, s), T2_EPI_WARPS / 2);  // one elected arrival per consumer warp of h
+            }
         mbar_init(bar_w, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
@@ -143,12 +199,12 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
     constexpr int NOPS = PRO == PRO_BNBWD ? 2 : 1;
     float4 q[PF][NOPS][4];
     const int pt = t - T2_EPI_WARPS * 32;  // producer thread id 0..255 (negative: consumers)
+    const int ph = pt >> 7, pq = pt & 127;  // producer warpgroup = half of the tile it fills, thread in it
     auto load = [&](int64_t tile, int kc, float4 (&dst)[NOPS][4]) {
         const int64_t m0 = tile * T2_BM;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            const int i = pt + 256 * j;
-            const int row = i >> 3, c16 = i & 7;
+            const int row = ph * 64 + (pq >> 3) + 16 * j, c16 = pq & 7;
             const bool ok = tile < tiles && m0 + row < p.M;
             dst[0][j] = ok ? __ldg(reinterpret_cast<const float4*>(p.A + (m0 + row) * p.lda + kc * T2_KC + c16 * 4))
                            : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -212,11 +268,11 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
         int64_t tile = blockIdx.x;
         int kc = 0;
         uint32_t it = 0;
-        const int c16 = pt & 7;  // 16-byte chunk of the 128-byte K row (same for all 4 rows)
+        const int c16 = pq & 7;  // 16-byte chunk of the 128-byte K row (same for all 4 rows)
         uint32_t soff[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) soff[j] = sw128_off((pt >> 3) + 32 * j, c16);
-        const uint32_t smem_u = smem_u32(smem);
+        for (int j = 0; j < 4; ++j) soff[j] = sw128_off((pq >> 3) + 16 * j, c16);
+        const uint32_t ring_u = ring(ph);
         const bool side_store = PRO == PRO_BNBWD && p.dy_out != nullptr && blockIdx.y == 0;
         auto st_shared4 = [](uint32_t addr, uint4 v) {
             asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y),
@@ -236,13 +292,13 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
                 cy = *reinterpret_cast<const float4*>(cy_s + col);
                 c0 = *reinterpret_cast<const float4*>(c0_s + col);
             }
-            if (use > 0) mbar_wait(bar_empty(s), (use - 1) & 1);
-            const uint32_t stage = smem_u + (uint32_t)s * T2_STAGE_BYTES;
-            const int64_t m0 = tile * T2_BM;
+            if (use > 0) mbar_wait(bar_empty(ph, s), (use - 1) & 1);
+            const uint32_t stage = ring_u + (uint32_t)s * T2_HALF_STAGE_BYTES;
+            const int64_t m0 = tile * T2_BM + ph * 64;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 float4 v = cur[0][j];
-                const int64_t row = m0 + (pt >> 3) + 32 * j;
+                const int64_t row = m0 + (pq >> 3) + 16 * j;
                 if (pro && row < p.M) {
                     if (PRO == PRO_BNBWD) {
                         const float4 y = cur[NOPS - 1][j];
@@ -256,8 +312,7 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
                         v.y = fmaf(sc.y, v.y, fmaf(cy.y, y.y, c0.y));
                         v.z = fmaf(sc.z, v.z, fmaf(cy.z, y.z, c0.z));
                         v.w = fmaf(sc.w, v.w, fmaf(cy.w, y.w, c0.w));
-                        if (side_store)
-                            *reinterpret_cast<float4*>(p.dy_out + row * p.lddy + col) = v;
+                        st_global4(p.dy_out + row * p.lddy + col, v, side_store);
                     } else {
                         v.x = fmaf(v.x, sc.x, sh.x);
                         v.y = fmaf(v.y, sc.y, sh.y);
@@ -281,11 +336,11 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
                 lo.z = to_tf32(v.z - __uint_as_float(hi.z));
                 lo.w = to_tf32(v.w - __uint_as_float(hi.w));
                 st_shared4(stage + soff[j], hi);
-                st_shared4(stage + T2_A_BYTES + soff[j], lo);
+                st_shared4(stage + T2_HALF_A_BYTES + soff[j], lo);
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncwarp();
-            if (lane == 0) mbar_arrive(bar_full(s));
+            if (lane == 0) mbar_arrive(bar_full(ph, s));
             advance(tile, kc);
             ++it;
         };
@@ -302,16 +357,20 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
         const int r = lane >> 2, cq = 2 * (lane & 3);
         float* acc_w = acc_s + warp * (NS * 4);
         const uint32_t wres_u32 = smem_u32(wres);
-        const uint32_t smem_u = smem_u32(smem);
+        const uint32_t ring_u = ring(g);
         float acc[NS / 2];
+        float n_w = 0.f;  // STATS: rows this warp has reduced so far (the count of every one of its columns)
         uint32_t it = 0;
         mbar_wait(bar_w, 0);  // resident weights have landed (TMA complete_tx)
         for (int64_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+            // warpgroup 1 waits for warpgroup 0 to have issued this tile's MMAs, warpgroup 0 (after its first
+            // tile) for warpgroup 1 to have issued the previous tile's
+            if (g == 1 || tile != blockIdx.x) turn_wait(T2_TURN_BAR + g);
             for (int kc = 0; kc < nk; ++kc, ++it) {
                 const int s = it % nst;
-                mbar_wait(bar_full(s), (it / nst) & 1);
-                const uint32_t a_hi = smem_u + (uint32_t)s * T2_STAGE_BYTES + (uint32_t)g * (64 * 128);
-                const uint32_t a_lo = a_hi + T2_A_BYTES;
+                mbar_wait(bar_full(g, s), (it / nst) & 1);
+                const uint32_t a_hi = ring_u + (uint32_t)s * T2_HALF_STAGE_BYTES;
+                const uint32_t a_lo = a_hi + T2_HALF_A_BYTES;
                 const uint32_t b_hi = wres_u32 + (uint32_t)(kc * 2) * (NS * T2_KC * 4);
                 const uint32_t b_lo = b_hi + NS * T2_KC * 4;
                 wg_reg_fence(acc);
@@ -329,85 +388,102 @@ tc_gemm2_kernel(const Tc2Args p, const __grid_constant__ CUtensorMap wmap) {
                 wg_wait<0>();
                 wg_reg_fence(acc);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(bar_empty(s));
+                if (lane == 0) mbar_arrive(bar_empty(g, s));
             }
+            // the other warpgroup's turn: warpgroup 1 takes this tile, warpgroup 0 the next one (if there is one;
+            // both walk the same tiles, so warpgroup 0 always waits for this)
+            if (g == 0 || tile + gridDim.x < tiles) turn_pass(T2_TURN_BAR + (g ^ 1));
             // ---- epilogue: this thread holds rows ra = row0 + r and rb = ra + 8, column pairs 8j + cq
             const int64_t row0 = tile * T2_BM + g * 64 + wl * 16;
             const int nv = (int)max((int64_t)0, min((int64_t)16, p.M - row0));
             const bool va = r < nv, vb = r + 8 < nv;
             float* ca = p.C + (row0 + r) * p.ldc + n0;
             float* cb = ca + 8 * p.ldc;
+            // STATS: the pivot of a column is the first value the warp saw in it, stored (lanes r == 0) at the
+            // first tile with a valid row and read by the whole warp at the later ones
+            const bool have_pivot = n_w > 0.f;
+            if (p.epi == EPI_STATS) __syncwarp();
+            const bool reduce = p.epi == EPI_BNRED || (p.epi == EPI_STATS && nv > 0);
+            // Blocks of 2 column pairs = the 4 columns 8(j0 + u) + cq + e, u < 2, e < 2, of this lane (block
+            // column k = 2u + e); lane r folds sum vr = 4(r & 1) + 2((r >> 1) & 1) + (r >> 2) of each block, i.e.
+            // the first (vr even) or second sum of block column vr / 2 (see reduce_scatter8)
+            const int vr = 4 * (r & 1) + 2 * ((r >> 1) & 1) + (r >> 2);
+            // BNRED reads the layer below's y for YB column pairs (two blocks; one at NS = 128, where the 64
+            // accumulators leave no room for more) ahead of their reductions
+            constexpr int YB = NS == 128 ? 2 : 4;
 #pragma unroll
-            for (int j = 0; j < NS / 8; ++j) {
-                const int c = 8 * j + cq;
-                const float2 oa = make_float2(acc[4 * j] + bias_s[c], acc[4 * j + 1] + bias_s[c + 1]);
-                const float2 ob = make_float2(acc[4 * j + 2] + bias_s[c], acc[4 * j + 3] + bias_s[c + 1]);
-                if (va) *reinterpret_cast<float2*>(ca + c) = oa;
-                if (vb) *reinterpret_cast<float2*>(cb + c) = ob;
+            for (int j1 = 0; j1 < NS / 8; j1 += YB) {
+                float2 ya[YB], yb[YB];
                 if (p.epi == EPI_BNRED) {
-                    // BatchNorm-backward sums of the layer below: gz = relu'(y) * g
-                    const float2 ya = va ? __ldg(reinterpret_cast<const float2*>(p.e_y + (row0 + r) * p.e_ldy + n0 + c))
-                                         : make_float2(0.f, 0.f);
-                    const float2 yb = vb ? __ldg(reinterpret_cast<const float2*>(p.e_y + (row0 + r + 8) * p.e_ldy + n0 + c))
-                                         : make_float2(0.f, 0.f);
-                    float b1[2], b2[2];
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const float esc = ev_s[c + e], esh = ev_s[NS + c + e];
-                        const float emu = ev_s[2 * NS + c + e], ers = ev_s[3 * NS + c + e];
-                        const float y0 = e ? ya.y : ya.x, y1 = e ? yb.y : yb.x;
-                        float g0 = va ? (e ? oa.y : oa.x) : 0.f, g1 = vb ? (e ? ob.y : ob.x) : 0.f;
-                        if (p.e_relu) {
-                            if (!(fmaf(y0, esc, esh) > 0.f)) g0 = 0.f;
-                            if (!(fmaf(y1, esc, esh) > 0.f)) g1 = 0.f;
-                        }
-                        b1[e] = g0 + g1;
-                        b2[e] = fmaf(g1, (y1 - emu) * ers, g0 * ((y0 - emu) * ers));
+                    for (int u = 0; u < YB; ++u) {
+                        const int64_t col = n0 + 8 * (j1 + u) + cq;
+                        ya[u] = va ? __ldg(reinterpret_cast<const float2*>(p.e_y + (row0 + r) * p.e_ldy + col))
+                                   : make_float2(0.f, 0.f);
+                        yb[u] = vb ? __ldg(reinterpret_cast<const float2*>(p.e_y + (row0 + r + 8) * p.e_ldy + col))
+                                   : make_float2(0.f, 0.f);
                     }
-                    // lanes with the same lane % 4 hold the same columns: fold the 8 row pairs
+                }
 #pragma unroll
-                    for (int e = 0; e < 2; ++e)
+                for (int j0 = j1; j0 < j1 + YB; j0 += 2) {
+                    float v[8];    // per block column k: the two sums over this thread's rows, at 2k and 2k + 1
+                    float piv[4];  // STATS: pivot of block column k
 #pragma unroll
-                        for (int o = 4; o < 32; o <<= 1) {
-                            b1[e] += __shfl_xor_sync(0xffffffffu, b1[e], o);
-                            b2[e] += __shfl_xor_sync(0xffffffffu, b2[e], o);
-                        }
-                    if (r == 0) {
+                    for (int u = 0; u < 2; ++u) {
+                        const int j = j0 + u;
+                        const int c = 8 * j + cq;
+                        const float2 oa = make_float2(acc[4 * j] + bias_s[c], acc[4 * j + 1] + bias_s[c + 1]);
+                        const float2 ob = make_float2(acc[4 * j + 2] + bias_s[c], acc[4 * j + 3] + bias_s[c + 1]);
+                        st_global2(ca + c, oa, va);
+                        st_global2(cb + c, ob, vb);
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
-                            float* o = acc_w + (c + e) * 4;
-                            o[0] += b1[e];
-                            o[1] += b2[e];
+                            const int k = 2 * u + e;
+                            if (p.epi == EPI_BNRED) {
+                                // BatchNorm-backward sums of the layer below: gz = relu'(y) * g
+                                const float esc = ev_s[c + e], esh = ev_s[NS + c + e];
+                                const float emu = ev_s[2 * NS + c + e], ers = ev_s[3 * NS + c + e];
+                                const float2 y0p = ya[j - j1], y1p = yb[j - j1];
+                                const float y0 = e ? y0p.y : y0p.x, y1 = e ? y1p.y : y1p.x;
+                                float g0 = va ? (e ? oa.y : oa.x) : 0.f, g1 = vb ? (e ? ob.y : ob.x) : 0.f;
+                                if (p.e_relu) {
+                                    if (!(fmaf(y0, esc, esh) > 0.f)) g0 = 0.f;
+                                    if (!(fmaf(y1, esc, esh) > 0.f)) g1 = 0.f;
+                                }
+                                v[2 * k] = g0 + g1;
+                                v[2 * k + 1] = fmaf(g1, (y1 - emu) * ers, g0 * ((y0 - emu) * ers));
+                            } else if (p.epi == EPI_STATS && nv > 0) {
+                                // pivoted sums over the valid rows of this warp's 16-row group
+                                const float x0 = e ? oa.y : oa.x, x1 = e ? ob.y : ob.x;
+                                const float first = __shfl_sync(0xffffffffu, x0, lane & 3);
+                                piv[k] = have_pivot ? acc_w[(c + e) * 4 + 3] : first;
+                                const float d0 = va ? x0 - piv[k] : 0.f;
+                                const float d1 = vb ? x1 - piv[k] : 0.f;
+                                v[2 * k] = d0 + d1;
+                                v[2 * k + 1] = fmaf(d1, d1, d0 * d0);
+                            }
+                        }
+                    }
+                    if (reduce) {
+                        // lanes with the same lane % 4 hold the same columns: fold the 8 row pairs
+                        const float sum = reduce_scatter8(v, r);
+                        const int k = vr >> 1;  // block column
+                        // BNRED: s1, s2 in o[0], o[1]; STATS: the pivoted sums in o[1], o[2] (o[0]: count, o[3]: pivot)
+                        acc_w[(8 * (j0 + (k >> 1)) + cq + (k & 1)) * 4 + (p.epi == EPI_STATS) + (vr & 1)] += sum;
+                        if (p.epi == EPI_STATS && r == 0 && !have_pivot) {
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) acc_w[(8 * (j0 + (q >> 1)) + cq + (q & 1)) * 4 + 3] = piv[q];
                         }
                     }
                 }
-                if (p.epi == EPI_STATS && nv > 0) {
-                    // per-column pivoted sums over the valid rows of this warp's 16-row group; the pivot
-                    // is the first value the warp ever saw in this column (kept across tiles)
+            }
+            if (p.epi == EPI_STATS && nv > 0) n_w += (float)nv;
+        }
+        if (p.epi == EPI_STATS && r == 0) {
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        float* o = acc_w + (c + e) * 4;
-                        const float n_old = o[0];
-                        const float first = __shfl_sync(0xffffffffu, e ? oa.y : oa.x, lane & 3);
-                        const float pivot = n_old > 0.f ? o[3] : first;
-                        const float d0 = va ? (e ? oa.y : oa.x) - pivot : 0.f;
-                        const float d1 = vb ? (e ? ob.y : ob.x) - pivot : 0.f;
-                        float s1 = d0 + d1, s2 = fmaf(d1, d1, d0 * d0);
-#pragma unroll
-                        for (int sh = 4; sh < 32; sh <<= 1) {
-                            s1 += __shfl_xor_sync(0xffffffffu, s1, sh);
-                            s2 += __shfl_xor_sync(0xffffffffu, s2, sh);
-                        }
-                        __syncwarp();
-                        if (r == 0) {
-                            o[0] = n_old + (float)nv;
-                            o[1] += s1;
-                            o[2] += s2;
-                            o[3] = pivot;
-                        }
-                        __syncwarp();
-                    }
-                }
+            for (int j = 0; j < NS / 8; ++j) {
+                acc_w[(8 * j + cq) * 4] = n_w;
+                acc_w[(8 * j + cq + 1) * 4] = n_w;
             }
         }
     }
