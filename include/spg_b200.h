@@ -667,6 +667,56 @@ int spg_lp_perfect_prediction(const int64_t* comp_ptr, const int64_t* point_ids,
                               const int64_t* labels, int64_t ld_labels, int n_classes, int64_t n_ver, int64_t* pred,
                               spg_stream_t stream);
 
+/* ---------------------------------------------------------------- learned-partition batch builder
+ * graph_loader + graph_collate of the learned-embedding branch, one call per file of the batch, each writing
+ * that file's slice of the collated outputs.  ref: supervized_partition/graph_processing.py:347-472,534-546.
+ *
+ * lp_augment: rgb_out [n, 3] = rgb / 255; xyz_out [n, 3] = xyz, or with rot (device float [9]: the float32
+ * rotation M row-major) ((p - ref) M) + ref with ref = (x, y, 0) of vertex ref_index and p = xyz with the z
+ * of vertex ref_index set to 0 (the reference's ref_point is a view of xyz).  Then jitter: xyz_out += noise and,
+ * with rgb_jitter, rgb_out = clip(rgb_out + noise, -1, 1); the noise is noise_xyz / noise_rgb [n, 3] (host
+ * draws, already clipped) or, with device_noise, clip(sigma N(0, 1), -clip, clip) from Philox4x32-10 keyed by
+ * seed, counter (vertex, file_pos, 0 for xyz / 1 for rgb).  No jitter when both are absent, and then
+ * rgb_jitter is ignored (rgb is jittered only with xyz).
+ * ref: graph_processing.py:353,534-546                                                                    */
+int spg_lp_augment(const float* xyz, const float* rgb, int64_t n_ver, const float* rot, int64_t ref_index,
+                   const float* noise_xyz, const float* noise_rgb, int device_noise, int rgb_jitter, float sigma,
+                   float clip, int64_t seed, int64_t file_pos, float* xyz_out, float* rgb_out, spg_stream_t stream);
+/* lp_subgraph_select: with a vertex mask [n] (uint8), new_index [n + 1] = exclusive scan of the mask (the new
+ * id of every kept vertex, the kept count last), selected [count] = the kept vertices in increasing order,
+ * edge_pos [E + 1] = exclusive scan of the edge mask mask[src] * mask[tgt] (the kept edge count last).
+ * object_max [1] = max over the kept vertices (every vertex without a mask) of objects, as the uint32
+ * id ^ 0x80000000.  Workspace from spg_lp_subgraph_workspace, 256-byte aligned.
+ * ref: graph_processing.py:371-385, partition/ply_c/random_subgraph.cpp:91-95                            */
+int spg_lp_subgraph_workspace(int64_t n_ver, int64_t n_edges, int64_t* bytes);
+int spg_lp_subgraph_select(const uint8_t* mask, const int32_t* objects, int64_t n_ver, const int32_t* src,
+                           const int32_t* tgt, int64_t n_edges, int32_t* new_index, int32_t* selected,
+                           int32_t* edge_pos, uint32_t* object_max, void* workspace, int64_t workspace_bytes,
+                           spg_stream_t stream);
+/* lp_subgraph_edges: the kept edges in their order (all edges when new_index is NULL), renumbered through
+ * new_index and shifted by vertex_offset (graph_collate :464-465), with their is_transition.
+ * ref: graph_processing.py:378-381,457-465                                                               */
+int spg_lp_subgraph_edges(const int32_t* src, const int32_t* tgt, const uint8_t* is_transition, int64_t n_edges,
+                          const int32_t* new_index, const int32_t* edge_pos, int64_t vertex_offset, int64_t* src_out,
+                          int64_t* tgt_out, uint8_t* is_transition_out, spg_stream_t stream);
+/* lp_object_offsets: offsets [B] = running sum of the object maxima of the earlier files (max, not max + 1,
+ * as graph_collate); a file with counts[b] == 0 kept vertices adds 0.  ref: graph_processing.py:447,467   */
+int spg_lp_object_offsets(const uint32_t* object_max, const int64_t* counts, int64_t n_files, int64_t* offsets,
+                          spg_stream_t stream);
+/* lp_local_clouds: for every kept vertex i (v = selected[i], or i when NULL) with its k first neighbours
+ * u_j = local_geometry[v, j] (original ids): diameter = sqrt((var_x + var_y) + var_z) of xyz[u_j] (numpy's
+ * sequential fp32 mean and variance), clouds [n_sel, 3 + 3 use_rgb, k] = (xyz[u_j] - xyz[v]) / (diameter +
+ * 1e-10) and rgb[u_j]; clouds_global [n_sel, ld_global] = [diameter | elevation (flag 1) | rgb[v] (2) |
+ * xyn[v] (4) | xyz[v, :2] (8)]; xyz_out [n_sel, 3], labels_out [n_sel, n_label_cols] (int64),
+ * objects_out [n_sel] = objects[v] + object_offset[0].  rgb_scale: rgb is the resident 0..255 array.
+ * k <= 256.  ref: graph_processing.py:387-411,430                                                         */
+int spg_lp_local_clouds(const float* xyz, const float* rgb, int rgb_scale, const int32_t* local_geometry,
+                        int64_t ld_geometry, int k, const int32_t* selected, int64_t n_sel, const float* elevation,
+                        const float* xyn, const int32_t* labels, int64_t n_label_cols, const int32_t* objects,
+                        const int64_t* object_offset, int use_rgb, int global_flags, float* clouds,
+                        float* clouds_global, int64_t ld_global, float* xyz_out, int64_t* labels_out,
+                        int64_t* objects_out, spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -76,6 +76,9 @@ enum KernelId {
     K_LP_WEIGHTS,
     K_LP_RELAX,
     K_LP_METRICS,
+    K_LP_AUGMENT,
+    K_LP_SUBGRAPH,
+    K_LP_LOCAL_CLOUDS,
     K_COUNT
 };
 

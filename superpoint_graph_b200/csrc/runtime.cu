@@ -29,6 +29,7 @@ static const char* kKernelNames[K_COUNT] = {
     "lp_incidence",      "lp_dist_fwd",        "lp_dist_bwd",         "lp_loss_fwd",
     "lp_loss_bwd",       "lp_cc",              "lp_xpart",            "lp_seal",
     "lp_weights",        "lp_relax",           "lp_metrics",
+    "lp_augment",        "lp_subgraph",        "lp_local_clouds",
 };
 
 struct Record {

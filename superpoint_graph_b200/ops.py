@@ -1280,3 +1280,60 @@ def lp_perfect_prediction(comp_ptr, point_ids, labels, n_ver):
     _lib.call("spg_lp_perfect_prediction", comp_ptr, point_ids, comp_ptr.numel() - 1, labels, labels.shape[1],
               labels.shape[1] - 1, n_ver, pred, _lib.current_stream())
     return pred
+
+
+# ------------------------------------------------------------- learned-partition batch builder
+LPL_GLOBAL_E, LPL_GLOBAL_RGB, LPL_GLOBAL_XYN, LPL_GLOBAL_XY = 1, 2, 4, 8
+
+
+def lp_augment(xyz, rgb, rot, ref_index, noise_xyz, noise_rgb, device_noise, rgb_jitter, sigma, clip, seed,
+               file_pos, xyz_out, rgb_out):
+    """rgb / 255, rotation about the reference point and jitter of one file (ref: graph_processing.py:353,
+    534-546); see include/spg_b200.h spg_lp_augment."""
+    _need_cuda(xyz, rgb, rot, noise_xyz, noise_rgb, xyz_out, rgb_out)
+    assert xyz.dtype == torch.float32 and rgb.dtype == torch.float32 and xyz.is_contiguous() and rgb.is_contiguous()
+    assert rot is None or (rot.dtype == torch.float32 and rot.numel() == 9 and rot.is_contiguous())
+    _lib.call("spg_lp_augment", xyz, rgb, xyz.shape[0], rot, int(ref_index), noise_xyz, noise_rgb,
+              int(bool(device_noise)), int(bool(rgb_jitter)), float(sigma), float(clip), int(seed), int(file_pos),
+              xyz_out, rgb_out, _lib.current_stream())
+
+
+def lp_subgraph_select(mask, objects, src, tgt, new_index, selected, edge_pos, object_max):
+    """Vertex / edge scans of a sub-graph mask and the object maximum (mask None: maximum only); see
+    spg_lp_subgraph_select."""
+    _need_cuda(mask, objects, src, tgt, new_index, selected, edge_pos, object_max)
+    n, E = objects.numel(), src.numel()
+    ws, nb = None, 0
+    if mask is not None:
+        nbytes = torch.zeros(1, dtype=torch.int64)
+        _lib.call("spg_lp_subgraph_workspace", n, E, nbytes)
+        ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=objects.device)
+        nb = ws.numel()
+    _lib.call("spg_lp_subgraph_select", mask, objects, n, src, tgt, E, new_index, selected, edge_pos, object_max, ws,
+              nb, _lib.current_stream())
+
+
+def lp_subgraph_edges(src, tgt, is_transition, new_index, edge_pos, vertex_offset, src_out, tgt_out, tr_out):
+    _need_cuda(src, tgt, is_transition, new_index, edge_pos, src_out, tgt_out, tr_out)
+    _lib.call("spg_lp_subgraph_edges", src, tgt, is_transition, src.numel(), new_index, edge_pos, int(vertex_offset),
+              src_out, tgt_out, tr_out, _lib.current_stream())
+
+
+def lp_object_offsets(object_max, counts, offsets):
+    _need_cuda(object_max, counts, offsets)
+    assert counts.dtype == torch.int64 and offsets.dtype == torch.int64
+    _lib.call("spg_lp_object_offsets", object_max, counts, counts.numel(), offsets, _lib.current_stream())
+
+
+def lp_local_clouds(xyz, rgb, rgb_scale, local_geometry, k, selected, n_sel, elevation, xyn, labels, objects,
+                    object_offset, use_rgb, global_flags, clouds, clouds_global, xyz_out, labels_out, objects_out):
+    """Local clouds, global features and gathered rows of one file's kept vertices (ref: graph_processing.py:
+    387-411,430); every output is that file's slice of the batch."""
+    _need_cuda(xyz, rgb, local_geometry, selected, elevation, xyn, labels, objects, object_offset, clouds,
+               clouds_global, xyz_out, labels_out, objects_out)
+    assert local_geometry.dtype == torch.int32 and local_geometry.is_contiguous()
+    assert clouds.dtype == torch.float32 and clouds.is_contiguous() and clouds_global.is_contiguous()
+    _lib.call("spg_lp_local_clouds", xyz, rgb, int(bool(rgb_scale)), local_geometry, local_geometry.shape[1], int(k),
+              selected, int(n_sel), elevation, xyn, labels, labels.shape[1], objects, object_offset,
+              int(bool(use_rgb)), int(global_flags), clouds, clouds_global, clouds_global.shape[1], xyz_out,
+              labels_out, objects_out, _lib.current_stream())

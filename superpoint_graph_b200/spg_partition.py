@@ -158,11 +158,19 @@ def compute_partition(args, embeddings, edg_source, edg_target, diff, xyz=0):
     ver_value = embeddings.detach().cpu().numpy().astype("f4")
     use_spatial = 0
     if args.spatial_emb > 0:
-        ver_value = np.hstack((ver_value, args.spatial_emb * xyz))
+        ver_value = np.hstack((ver_value, args.spatial_emb * _host(xyz, "f4")))
         use_spatial = 1
-    return libcp.cutpursuit(ver_value, np.asarray(edg_source).astype("uint32"), np.asarray(edg_target).astype("uint32"),
+    return libcp.cutpursuit(ver_value, _host(edg_source, "uint32"), _host(edg_target, "uint32"),
                             edge_weight, args.reg_strength / (4 * args.k_nn_adj), cutoff=args.CP_cutoff,
                             spatial=use_spatial, weight_decay=0.7)
+
+
+def _host(x, dtype):
+    """Host copy for libcp: tensors (CUDA ones included, e.g. a load_batch batch) are copied and cast to `dtype`;
+    numpy arrays go through as before (edges cast to uint32, xyz as given)."""
+    if torch.is_tensor(x):
+        return x.detach().cpu().numpy().astype(dtype)
+    return np.asarray(x).astype(dtype) if dtype == "uint32" else x
 
 
 def compute_weights_SEAL(pred_components, pred_in_component, objects, edg_source, edg_target, is_transition,
