@@ -717,6 +717,36 @@ int spg_lp_local_clouds(const float* xyz, const float* rgb, int rgb_scale, const
                         float* clouds_global, int64_t ld_global, float* xyz_out, int64_t* labels_out,
                         int64_t* objects_out, spg_stream_t stream);
 
+/* ---------------------------------------------------------------- k-NN graphs and geometric features
+ * compute_graph_nn / compute_graph_nn_2 / compute_geof of the partition pipelines (ref: partition/graphs.py:11-70,
+ * partition/ply_c/ply_c.cpp:384-462), xyz float32 [n, 3] on the device, n < 2^31 - 1.
+ *
+ * spg_knn_bounds: words [8] (device, uint32) = the order-preserving keys of the finite coordinates' minimum
+ * (words 0-2) and maximum (3-5) per axis, status (6) = 1 if some coordinate is not finite.
+ * spg_knn_grid: a grid of cubic cells of size `cell` from origin (ox, oy, oz), dim_* cells per axis (each
+ * < 2^21, coordinates outside are clamped into the edge cells): the stable sort of the points by cell and the
+ * occupied-cell table, into `workspace` (spg_knn_workspace bytes, 256-byte aligned); n_cells [1] (device) = the
+ * number of occupied cells.  The grid only sets the work of the query, never its result.
+ * spg_knn_query (same grid arguments and workspace): for every vertex i its k <= spg_knn_max_k() nearest other
+ * vertices ranked by d2 = (dx dx + dy dy) + dz dz in float64 (dx = double(x_i) - double(x_j)), ties by the smaller
+ * index; source, target [n k1] (int64) = i, the first k1 of them; distances [n k1] = float32(sqrt(d2));
+ * target2 [n k] (may be NULL) = all k.  Needs n >= k + 1.
+ * spg_geof: geof [n, 4] (float32, 16-byte aligned) = linearity, planarity, scattering, verticality of vertex i
+ * and its k neighbours target[i k .. i k + k) (int64): fp64 mean and covariance / (k + 1), symmetric fp64
+ * eigen-solve, eigenvalues sorted descending and clamped at 0, ply_c.cpp:436-446 in fp64 (NaN in all four where
+ * the largest eigenvalue is 0); status [1] (device, uint32) = 2 and the row NaN where an id is outside [0, n). */
+int spg_knn_max_k(void);
+int spg_knn_workspace(int64_t n, int64_t* bytes);
+int spg_knn_bounds(const float* xyz, int64_t n, uint32_t* words, spg_stream_t stream);
+int spg_knn_grid(const float* xyz, int64_t n, double ox, double oy, double oz, double cell, int64_t dim_x,
+                 int64_t dim_y, int64_t dim_z, void* workspace, int64_t workspace_bytes, int32_t* n_cells,
+                 spg_stream_t stream);
+int spg_knn_query(int64_t n, int k, int k1, double ox, double oy, double oz, double cell, int64_t dim_x,
+                  int64_t dim_y, int64_t dim_z, const void* workspace, int64_t workspace_bytes, int64_t* source,
+                  int64_t* target, float* distances, int64_t* target2, spg_stream_t stream);
+int spg_geof(const float* xyz, int64_t n, const int64_t* target, int k, float* geof, uint32_t* status,
+             spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

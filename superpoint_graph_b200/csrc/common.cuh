@@ -79,6 +79,10 @@ enum KernelId {
     K_LP_AUGMENT,
     K_LP_SUBGRAPH,
     K_LP_LOCAL_CLOUDS,
+    K_GEO_BOUNDS,
+    K_GEO_GRID,
+    K_GEO_KNN,
+    K_GEO_GEOF,
     K_COUNT
 };
 

@@ -30,6 +30,7 @@ static const char* kKernelNames[K_COUNT] = {
     "lp_loss_bwd",       "lp_cc",              "lp_xpart",            "lp_seal",
     "lp_weights",        "lp_relax",           "lp_metrics",
     "lp_augment",        "lp_subgraph",        "lp_local_clouds",
+    "geo_bounds",        "geo_grid",           "geo_knn",             "geo_geof",
 };
 
 struct Record {

@@ -1337,3 +1337,62 @@ def lp_local_clouds(xyz, rgb, rgb_scale, local_geometry, k, selected, n_sel, ele
               selected, int(n_sel), elevation, xyn, labels, labels.shape[1], objects, object_offset,
               int(bool(use_rgb)), int(global_flags), clouds, clouds_global, clouds_global.shape[1], xyz_out,
               labels_out, objects_out, _lib.current_stream())
+
+
+# ------------------------------------------------------------- k-NN graphs and geometric features
+def knn_max_k():
+    return int(_lib.lib().spg_knn_max_k())
+
+
+def knn_bounds(xyz):
+    """int32 [8] on the device: the order-preserving keys of the per-axis minimum (0-2) and maximum (3-5) of the
+    finite coordinates, and the status word (6; 1: a non-finite coordinate); see spg_knn_bounds."""
+    _need_cuda(xyz)
+    assert xyz.dtype == torch.float32 and xyz.is_contiguous()
+    words = torch.empty(8, dtype=torch.int32, device=xyz.device)
+    _lib.call("spg_knn_bounds", xyz, xyz.shape[0], words, _lib.current_stream())
+    return words
+
+
+def knn_workspace(n, device):
+    nbytes = torch.zeros(1, dtype=torch.int64)
+    _lib.call("spg_knn_workspace", int(n), nbytes)
+    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
+
+
+def knn_grid(xyz, grid, ws):
+    """Sorts the cloud into the cells of grid = (ox, oy, oz, cell, dim_x, dim_y, dim_z) inside `ws`; returns the
+    number of occupied cells, int32 [1] on the device."""
+    _need_cuda(xyz, ws)
+    n_cells = torch.empty(1, dtype=torch.int32, device=xyz.device)
+    ox, oy, oz, cell, dx, dy, dz = grid
+    _lib.call("spg_knn_grid", xyz, xyz.shape[0], float(ox), float(oy), float(oz), float(cell), int(dx), int(dy),
+              int(dz), ws, ws.numel(), n_cells, _lib.current_stream())
+    return n_cells
+
+
+def knn_query(n, k, k1, grid, ws, want_target2):
+    """(source, target int64 [n k1], distances float32 [n k1], target2 int64 [n k] or None) from the sorted cloud
+    that knn_grid left in `ws`."""
+    _need_cuda(ws)
+    dev = ws.device
+    source = torch.empty(n * k1, dtype=torch.int64, device=dev)
+    target = torch.empty(n * k1, dtype=torch.int64, device=dev)
+    distances = torch.empty(n * k1, dtype=torch.float32, device=dev)
+    target2 = torch.empty(n * k, dtype=torch.int64, device=dev) if want_target2 else None
+    ox, oy, oz, cell, dx, dy, dz = grid
+    _lib.call("spg_knn_query", int(n), int(k), int(k1), float(ox), float(oy), float(oz), float(cell), int(dx),
+              int(dy), int(dz), ws, ws.numel(), source, target, distances, target2, _lib.current_stream())
+    return source, target, distances, target2
+
+
+def geof(xyz, target, k):
+    """(geof float32 [n, 4], status int32 [1] on the device; 2: an id outside [0, n)); see spg_geof."""
+    _need_cuda(xyz, target)
+    assert xyz.dtype == torch.float32 and xyz.is_contiguous()
+    assert target.dtype == torch.int64 and target.is_contiguous()
+    n = xyz.shape[0]
+    out = torch.empty((n, 4), dtype=torch.float32, device=xyz.device)
+    status = torch.empty(1, dtype=torch.int32, device=xyz.device)
+    _lib.call("spg_geof", xyz, n, target, int(k), out, status, _lib.current_stream())
+    return out, status
