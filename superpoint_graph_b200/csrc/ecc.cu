@@ -11,27 +11,15 @@
 // source-sorted CSR so that no atomics are needed (deterministic).
 //
 // HBM-bound integer/float streaming work: no tensor cores on purpose.
-#include "common.cuh"
+#include "ecc_rows.cuh"
 
 namespace spg {
 
 // ------------------------------------------------------------------ fast paths
 // C == 32, float32, no idxe.  A row of x / w(vv) / out is 128 B = 8 lanes x float4.
 
-constexpr int kC = 32;
-constexpr int kG = kC / 4;  // lanes per row
-
-__device__ __forceinline__ float4 fma4(float4 a, float4 b, float4 c) {
-    c.x = fmaf(a.x, b.x, c.x);
-    c.y = fmaf(a.y, b.y, c.y);
-    c.z = fmaf(a.z, b.z, c.z);
-    c.w = fmaf(a.w, b.w, c.w);
-    return c;
-}
-
-// One warp per target node: lane = (slot = lane>>3, sub = lane&7); the 4 slots walk the node's
-// edges interleaved (4 independent gather chains per node, 2 edges in flight per slot), the 8 sub
-// lanes cover the 32 channels with float4.  Slot partials are combined with two shuffles.
+// Vector filters: one warp per target node (ecc_rows.cuh).  x is read through the non-coherent
+// path, the filter bank is streamed.
 __global__ void __launch_bounds__(256)
 ecc_vv_fwd_kernel(const float4* __restrict__ x, const float4* __restrict__ w,
                   const int* __restrict__ rowptr, const int* __restrict__ idxn,
@@ -40,43 +28,9 @@ ecc_vv_fwd_kernel(const float4* __restrict__ x, const float4* __restrict__ w,
     const int lane = threadIdx.x & 31;
     const int64_t node = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (node >= n_out) return;
-    const int slot = lane >> 3, sub = lane & 7;
-    const int beg = rowptr[node], end = rowptr[node + 1];
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    int e = beg + slot;
-    for (; e + 4 < end; e += 8) {
-        const int s0 = __ldg(idxn + e), s1 = __ldg(idxn + e + 4);
-        const float4 w0 = ld_stream4(w + (int64_t)e * kG + sub);
-        const float4 w1 = ld_stream4(w + (int64_t)(e + 4) * kG + sub);
-        const float4 x0 = __ldg(x + (int64_t)s0 * kG + sub);
-        const float4 x1 = __ldg(x + (int64_t)s1 * kG + sub);
-        acc = fma4(x0, w0, acc);
-        acc = fma4(x1, w1, acc);
-    }
-    if (e < end) {
-        const int s0 = __ldg(idxn + e);
-        const float4 w0 = ld_stream4(w + (int64_t)e * kG + sub);
-        const float4 x0 = __ldg(x + (int64_t)s0 * kG + sub);
-        acc = fma4(x0, w0, acc);
-    }
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        acc.x += __shfl_xor_sync(0xffffffffu, acc.x, o);
-        acc.y += __shfl_xor_sync(0xffffffffu, acc.y, o);
-        acc.z += __shfl_xor_sync(0xffffffffu, acc.z, o);
-        acc.w += __shfl_xor_sync(0xffffffffu, acc.w, o);
-    }
-    if (slot == 0) {
-        const int deg = end - beg;
-        if (deg > 0) {
-            const float d = (float)deg;
-            acc.x /= d;
-            acc.y /= d;
-            acc.z /= d;
-            acc.w /= d;
-        }
-        out[node * kG + sub] = acc;
-    }
+    const float4 acc =
+        ecc_vv_row_fwd<LdNc, LdCs>((const float*)x, w, idxn, rowptr[node], rowptr[node + 1], lane);
+    if (lane < kG) out[node * kG + lane] = acc;  // slot 0: sub = lane
 }
 
 // Matrix filters W_e [32,32] (4 KB per edge): one warp per target node.  A warp
@@ -109,13 +63,7 @@ ecc_mat_fwd_kernel(const float* __restrict__ x, const float4* __restrict__ w,
             acc.w = fmaf(xk, wv[it].w, acc.w);
         }
     }
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        acc.x += __shfl_xor_sync(0xffffffffu, acc.x, o);
-        acc.y += __shfl_xor_sync(0xffffffffu, acc.y, o);
-        acc.z += __shfl_xor_sync(0xffffffffu, acc.z, o);
-        acc.w += __shfl_xor_sync(0xffffffffu, acc.w, o);
-    }
+    acc = slot_reduce(acc);
     if (r == 0) {
         const int deg = end - beg;
         if (deg > 0) {
@@ -219,7 +167,7 @@ ecc_mat_bwd_w_kernel(const float* __restrict__ xs, const float4* __restrict__ gs
 }
 
 // grad_x[j,:] = add0 + add1 + sum_{e out of j} w[e,:] * g[t_e,:]/deg_t  (vector filters)
-// warp per source node, 4 edge slots x 8 channel lanes (as the forward kernel).
+// warp per source node (ecc_rows.cuh); w and g through the non-coherent path.
 __global__ void __launch_bounds__(256)
 ecc_vv_bwd_x_kernel(const float4* __restrict__ w, const float4* __restrict__ g,
                     const int* __restrict__ tgt_rowptr, const int* __restrict__ src_rowptr,
@@ -230,44 +178,13 @@ ecc_vv_bwd_x_kernel(const float4* __restrict__ w, const float4* __restrict__ g,
     const int lane = threadIdx.x & 31;
     const int64_t node = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (node >= n_in) return;
-    const int slot = lane >> 3, sub = lane & 7;
-    const int beg = src_rowptr[node], end = src_rowptr[node + 1];
-    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int p = beg + slot; p < end; p += 4) {
-        const int e = __ldg(src_perm + p);
-        const int tg = __ldg(edge_tgt + e);
-        const float4 wv = __ldg(w + (int64_t)e * kG + sub);
-        const float inv = 1.f / (float)(__ldg(tgt_rowptr + tg + 1) - __ldg(tgt_rowptr + tg));
-        float4 gv = __ldg(g + (int64_t)tg * kG + sub);
-        gv.x *= inv;
-        gv.y *= inv;
-        gv.z *= inv;
-        gv.w *= inv;
-        acc = fma4(wv, gv, acc);
-    }
-#pragma unroll
-    for (int o = 8; o <= 16; o <<= 1) {
-        acc.x += __shfl_xor_sync(0xffffffffu, acc.x, o);
-        acc.y += __shfl_xor_sync(0xffffffffu, acc.y, o);
-        acc.z += __shfl_xor_sync(0xffffffffu, acc.z, o);
-        acc.w += __shfl_xor_sync(0xffffffffu, acc.w, o);
-    }
-    if (slot == 0) {
-        if (add0) {
-            const float4 a = add0[node * kG + sub];
-            acc.x += a.x;
-            acc.y += a.y;
-            acc.z += a.z;
-            acc.w += a.w;
-        }
-        if (add1) {
-            const float4 a = add1[node * kG + sub];
-            acc.x += a.x;
-            acc.y += a.y;
-            acc.z += a.z;
-            acc.w += a.w;
-        }
-        grad_x[node * kG + sub] = acc;
+    float4 acc = ecc_vv_row_bwd_x<LdNc, LdNc>(w, (const float*)g, tgt_rowptr, src_perm, edge_tgt,
+                                              src_rowptr[node], src_rowptr[node + 1], lane);
+    if (lane < kG) {  // slot 0: sub = lane
+        const int64_t o = node * kG + lane;
+        if (add0) acc = add4(acc, add0[o]);
+        if (add1) acc = add4(acc, add1[o]);
+        grad_x[o] = acc;
     }
 }
 

@@ -873,22 +873,25 @@ def test_graph_conv_module_matrix_filters(dev):
     close_grads({k: p.grad for k, p in fnet.named_parameters()}, {k: v.grad for k, v in sd.items()}, 3e-4)
 
 
-@pytest.mark.parametrize("n_nodes,cat_all", [(1024, False), (1024, True), (5000, True), (37, False)])
-def test_fused_recurrence_is_bit_identical_to_per_step_kernels(dev, monkeypatch, n_nodes, cat_all):
+@pytest.mark.parametrize("cat_all", [False, True])
+@pytest.mark.parametrize("n_nodes", [37, 1024, 5000])
+@pytest.mark.parametrize("cell", ["GRUCellEx", "LSTMCellEx"])
+def test_fused_recurrence_is_bit_identical_to_per_step_kernels(dev, monkeypatch, cell, n_nodes, cat_all):
     """One-kernel R x {ECC, cell} loop (grid barrier between steps) vs. the 2R / 3R separate
-    launches: same device functions, same summation order -> identical bits, forward and backward."""
-    from superpoint_graph_b200 import ops, synthetic
+    launches, for both cells: the ECC rows (ecc_rows.cuh) and the cell rows are the same device
+    functions in both paths, so the sums run in the same order -> identical bits, forward and
+    backward."""
+    from superpoint_graph_b200 import ops, spg_modules, synthetic
     from superpoint_graph_b200.spg_ecc import GraphConvInfo
     from superpoint_graph_b200.spg_graphnet import create_fnet
-    from superpoint_graph_b200.spg_modules import RNNGraphConvModule, GRUCellEx
     torch.manual_seed(3)
     b = synthetic.make_batch(n_nodes, k=8, seed=11, npts=8, minpts=4)
     gi = GraphConvInfo.from_arrays(b["idxn"].numpy(), b["degs"].numpy(), b["edgefeats"].numpy())
     gi.cuda()
     fnet = create_fnet([13, 32, 128, 64, 32], True, 0, 2)
-    mod = RNNGraphConvModule(GRUCellEx(32, 32, bias=True, layernorm=True, ingate=True), fnet, 32,
-                             vv=True, gc_info=gi, nrepeats=10, cat_all=cat_all, use_pyg=False,
-                             cuda=True).to(dev).train()
+    cell_mod = getattr(spg_modules, cell)(32, 32, bias=True, layernorm=True, ingate=True)
+    mod = spg_modules.RNNGraphConvModule(cell_mod, fnet, 32, vv=True, gc_info=gi, nrepeats=10,
+                                         cat_all=cat_all, use_pyg=False, cuda=True).to(dev).train()
     x0 = torch.randn(n_nodes, 32, device=dev)
     results = []
     for fused in (True, False):

@@ -3,8 +3,9 @@
 CPU: the oracle against lstm.npz, lstm_plain.npz and graphnet_lstm.npz (made by the unmodified reference),
 the model's state-dict layout, the drop-in name and the rejected use_pyg=1 path.
 GPU: the cell kernels against the golden and a float64 restatement at both rows-per-warp tilings and two
-widths, GraphNetwork against the golden (fused and per-step recurrence), the fused recurrence against the
-per-step kernels bit for bit, and the Trainer's steps, replays and inference graphs.
+widths, GraphNetwork against the golden (fused and per-step recurrence), and the Trainer's steps, replays
+and inference graphs.  The fused recurrence against the per-step kernels, bit for bit, is tested for both
+cells in test_gpu_parity.py.
 """
 import os
 
@@ -303,38 +304,6 @@ def test_graphnet_lstm_golden(golden_dir, dev, monkeypatch, i, fused):
     net.eval()
     with torch.no_grad():
         close(net(emb.detach()), g[tag + "out_eval"], 1e-4)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("cat_all", [False, True])
-@pytest.mark.parametrize("n_nodes", [37, 1024, 5000])
-def test_fused_lstm_recurrence_is_bit_identical_to_per_step_kernels(dev, monkeypatch, n_nodes, cat_all):
-    """One-kernel R x {ECC, LSTM cell} loop vs. the per-step launches: same device functions, same
-    summation order -> identical bits, forward and backward."""
-    from superpoint_graph_b200 import ops, synthetic
-    from superpoint_graph_b200.spg_ecc import GraphConvInfo
-    from superpoint_graph_b200.spg_graphnet import create_fnet
-    from superpoint_graph_b200.spg_modules import LSTMCellEx, RNNGraphConvModule
-    torch.manual_seed(3)
-    b = synthetic.make_batch(n_nodes, k=8, seed=11, npts=8, minpts=4)
-    gi = GraphConvInfo.from_arrays(b["idxn"].numpy(), b["degs"].numpy(), b["edgefeats"].numpy())
-    gi.cuda()
-    fnet = create_fnet([13, 32, 128, 64, 32], True, 0, 2)
-    mod = RNNGraphConvModule(LSTMCellEx(32, 32, bias=True, layernorm=True, ingate=True), fnet, 32,
-                             vv=True, gc_info=gi, nrepeats=10, cat_all=cat_all, use_pyg=False,
-                             cuda=True).to(dev).train()
-    x0 = torch.randn(n_nodes, 32, device=dev)
-    results = []
-    for fused in (True, False):
-        monkeypatch.setattr(ops, "USE_FUSED_RNN", [fused])
-        assert ops.rnn_vv_supported(torch.empty(1, 32, device=dev), gi.graph(), n_nodes, 32) == fused
-        mod.zero_grad()
-        x = x0.clone().requires_grad_(True)
-        y = mod(x)
-        (y * torch.linspace(-1, 1, y.numel(), device=dev).view_as(y)).sum().backward()
-        results.append([y.detach(), x.grad] + [p.grad.clone() for p in mod.parameters()])
-    for a, c in zip(*results):
-        assert torch.equal(a, c)
 
 
 TRAIN_CONFIGS = ["lstm_10_1_1_1_0,f_13", "lstm_2_0,f_13"]
