@@ -186,18 +186,6 @@ def test_gru_cell_golden(golden_dir, dev, name, ln, ig):
     close_grads({k: p.grad for k, p in cell.named_parameters()}, sub(g, "grad."))
 
 
-def test_gru_cell_ragged_rows(dev):
-    """Row counts that are not multiples of the warp tile, vs the oracle."""
-    from superpoint_graph_b200.spg_modules import GRUCellEx
-    torch.manual_seed(4)
-    cell = GRUCellEx(32, 32)
-    sd = {k: v.clone() for k, v in cell.state_dict().items()}
-    cell.to(dev)
-    for n in (1, 3, 33, 1027):
-        x, h = torch.randn(n, 32), torch.randn(n, 32)
-        close(cell(x.to(dev), h.to(dev)), nets_ref.gru_cell_ex(x, h, sd, ""))
-
-
 # ---------------------------------------------------------------------------------- dense
 @pytest.mark.parametrize("M,N,K", [(1, 1, 1), (257, 70, 13), (1000, 64, 14), (300, 257, 260), (4096, 32, 64)])
 def test_gemm_layouts(dev, M, N, K):

@@ -2,10 +2,10 @@
 
 CPU: the oracle against lstm.npz, lstm_plain.npz and graphnet_lstm.npz (made by the unmodified reference),
 the model's state-dict layout, the drop-in name and the rejected use_pyg=1 path.
-GPU: the cell kernels against the golden and a float64 restatement at both rows-per-warp tilings and two
-widths, GraphNetwork against the golden (fused and per-step recurrence), and the Trainer's steps, replays
-and inference graphs.  The fused recurrence against the per-step kernels, bit for bit, is tested for both
-cells in test_gpu_parity.py.
+GPU: the cell kernels against the golden, GraphNetwork against the golden (fused and per-step recurrence),
+and the Trainer's steps, replays and inference graphs.  The cell kernels at every width, tiling and option
+against float64 are tested for both cells in test_recurrent_widths.py, the fused recurrence against the
+per-step kernels, bit for bit, in test_gpu_parity.py.
 """
 import os
 
@@ -210,59 +210,6 @@ def test_lstm_cell_golden(golden_dir, dev, name, ln, ig):
     close(h.grad, g["gh"], 3e-4)
     close(c.grad, g["gcx"], 3e-4)
     close_grads({k: p.grad for k, p in cell.named_parameters()}, sub(g, "grad."), 3e-4)
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("H", [32, 64])
-@pytest.mark.parametrize("n", [1, 3, 33, 1027, 20000])
-def test_lstm_cell_vs_float64(dev, n, H):
-    """Row counts off the warp tile, both rows-per-warp tilings (20000 rows take 4 per warp at H = 32;
-    at H = 64 the weights leave room for 1 row per warp only), against float64."""
-    from superpoint_graph_b200.spg_modules import LSTMCellEx
-    torch.manual_seed(n + H)
-    cell = LSTMCellEx(H, H)
-    with torch.no_grad():
-        cell.bias_ih.normal_(0, 0.3)
-    sd = {k: v.clone() for k, v in cell.state_dict().items()}
-    cell.to(dev)
-    x, h, c, g, gc = (torch.randn(n, H) for _ in range(5))
-    hy_r, cy_r, gx_r, gh_r, gc_r, grads_r = _cell_oracle(sd, x, h, c, g, gc, True, True)
-    xd, hd, cd = (v.to(dev).requires_grad_(True) for v in (x, h, c))
-    hy, cy = cell(xd, (hd, cd))
-    close(hy, hy_r, 1e-4)
-    close(cy, cy_r, 1e-4)
-    ((hy * g.to(dev)).sum() + (cy * gc.to(dev)).sum()).backward()
-    close(xd.grad, gx_r, 3e-4)
-    close(hd.grad, gh_r, 3e-4)
-    close(cd.grad, gc_r, 3e-4)
-    close_grads({k: p.grad for k, p in cell.named_parameters()}, grads_r, 3e-4)
-
-
-@pytest.mark.gpu
-def test_cell_width_limits(dev):
-    """Rows per warp: the LSTM falls back to 1 row when 4 do not fit and is served up to H = 73 (weights plus
-    one row per warp in 227 KB); the GRU keeps its selection: 4 rows for >= 8448 rows, unsupported where
-    those do not fit (H = 80), 1 row below that count."""
-    from superpoint_graph_b200 import ops
-    flags = ops.GRU_LAYERNORM | ops.GRU_INGATE | ops.GRU_BIAS
-
-    def weights(G, H):
-        return [torch.randn(G * H, H, device=dev) * 0.1, torch.randn(G * H, H, device=dev) * 0.1,
-                torch.zeros(G * H, device=dev), torch.zeros(G * H, device=dev),
-                torch.randn(H, H, device=dev) * 0.1, torch.zeros(H, device=dev)]
-
-    for H, n in ((73, 9000), (73, 100)):
-        x = torch.randn(n, H, device=dev)
-        hy, cy = ops.lstm_fwd(x, x, x, *weights(4, H), flags)
-        assert torch.isfinite(hy).all() and torch.isfinite(cy).all()
-    x = torch.randn(100, 74, device=dev)
-    with pytest.raises(RuntimeError, match="not supported"):
-        ops.lstm_fwd(x, x, x, *weights(4, 74), flags)
-    x = torch.randn(100, 80, device=dev)
-    assert torch.isfinite(ops.gru_fwd(x, x, *weights(3, 80), flags)).all()
-    x = torch.randn(9000, 80, device=dev)
-    with pytest.raises(RuntimeError, match="not supported"):
-        ops.gru_fwd(x, x, *weights(3, 80), flags)
 
 
 @pytest.mark.gpu
