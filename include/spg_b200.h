@@ -536,6 +536,7 @@ int spg_allreduce_clamp_adam(const float* grad, float* const* peer_stage, uint32
  * for every superpoint b (n_points must be 128 = one tensor-core M tile, n_features <= 16):
  *   x = clouds[b] ([F, 128], NCL as the reference stacks them, learning/spg.py:162)
  *   if T: (x0, x1) <- (x0, x1) (T[b] (+ I))                                   (pointnet.py:123)
+ *         (T needs n_features >= 2: T with a single feature is SPG_E_BADARG)
  *   for l < n_layers: x <- relu(W_l x + b_l)     W_l [widths[l], K_l], BatchNorm already folded in
  *   pooled[b, :widths[n_layers-1]] = max over the 128 points
  * Activations stay in shared memory; the input tile and the weight stream arrive by TMA;

@@ -289,7 +289,7 @@ pointnet_fused_kernel(const PfArgs p, const __grid_constant__ CUtensorMap wmap,
             for (int f = 0; f < 16; ++f) v[f] = (fh == 0 && f < p.F) ? xin[f * PF_ROWS + row] : 0.f;
             __syncwarp();
             if (lane == 0) mbar_arrive(x_empty(xb));
-            if (fh == 0 && p.T && p.F >= 2) {
+            if (fh == 0 && p.T) {
                 const float eye = p.add_eye ? 1.f : 0.f;
                 const float t00 = p.T[b * 4 + 0] + eye, t01 = p.T[b * 4 + 1], t10 = p.T[b * 4 + 2],
                             t11 = p.T[b * 4 + 3] + eye;
@@ -443,6 +443,7 @@ int spg_pointnet_fused_eval(const float* clouds, int64_t n_clouds, int n_feature
     if (!spg_pointnet_fused_supported(n_features, n_points, n_layers, widths)) return SPG_E_UNSUPPORTED;
     if (n_clouds == 0) return SPG_OK;
     if (!clouds || !weight_image || !bias || !pooled || ldp < widths[n_layers - 1]) return SPG_E_BADARG;
+    if (T && n_features < 2) return SPG_E_BADARG;  // the transform acts on the (x, y) features
     if (((uintptr_t)clouds | (uintptr_t)weight_image) & 15) return SPG_E_ALIGN;
     if (n_clouds * n_features >= (1ll << 31)) return SPG_E_UNSUPPORTED;
     PfArgs a;
@@ -502,6 +503,7 @@ int spg_pointnet_fused_eval_bf16(const float* clouds, int64_t n_clouds, int n_fe
     if (!spg_pointnet_fused_supported(n_features, n_points, n_layers, widths)) return SPG_E_UNSUPPORTED;
     if (n_clouds == 0) return SPG_OK;
     if (!clouds || !weight_image || !bias || !pooled || ldp < widths[n_layers - 1]) return SPG_E_BADARG;
+    if (T && n_features < 2) return SPG_E_BADARG;  // the transform acts on the (x, y) features
     if (((uintptr_t)clouds | (uintptr_t)weight_image) & 15) return SPG_E_ALIGN;
     if (n_clouds * n_features >= (1ll << 31)) return SPG_E_UNSUPPORTED;
     PfArgs a;

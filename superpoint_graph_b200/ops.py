@@ -5,6 +5,7 @@ on torch's current stream.  CPU tensors are rejected: there is no CPU implementa
 product (the CPU restatement lives in oracle/ and is test infrastructure only).
 """
 import os
+import weakref
 
 import numpy as np
 import torch
@@ -54,6 +55,17 @@ def workspace(nfloats, device, slot=0):
         buf = torch.empty(max(int(nfloats), grow, 1 << 16), dtype=torch.float32, device=device)
         _workspaces[key] = buf
     return buf
+
+
+WEIGHTS_GENERATION = [0]
+
+
+def weights_written():
+    """Called by every wrapper that writes parameters or BatchNorm running statistics through a raw pointer
+    (the optimizer kernels, the BatchNorm folds given running statistics).  Such writes bump no tensor version
+    counter, so caches of values derived from the weights (the folded images of pointnet_fused_image) compare
+    this generation instead."""
+    WEIGHTS_GENERATION[0] += 1
 
 
 def zero_(t):
@@ -393,6 +405,8 @@ def _merge_stats(sws, tiles, N, M, dev, fold):
         _lib.call("spg_colstats_merge", sws, tiles, N, mean, var, _lib.current_stream())
         return mean, var
     gamma, beta, eps, rm, rv, nbt, mom = fold
+    if rm is not None:
+        weights_written()
     scale = torch.empty(N, dtype=torch.float32, device=dev)
     shift = torch.empty(N, dtype=torch.float32, device=dev)
     _lib.call("spg_colstats_merge_fold", sws, tiles, N, mean, var, gamma, beta, float(eps), scale, shift,
@@ -534,6 +548,8 @@ def tc_gemm(A, lda, W, ldw, transpose, M, N, K, bias=None, a_aff=None, stats=Fal
         var = torch.empty(N, dtype=torch.float32, device=dev)
         if fold is not None:
             gamma, beta, eps, rm, rv, nbt, mom = fold
+            if rm is not None:
+                weights_written()
             scale = torch.empty(N, dtype=torch.float32, device=dev)
             shift = torch.empty(N, dtype=torch.float32, device=dev)
     elif bnred is not None:
@@ -593,6 +609,8 @@ def _chunks(M):
 def bn_fold(mean, var, gamma, beta, eps, running_mean=None, running_var=None, momentum=0.1, M=0,
             num_batches_tracked=None):
     _need_cuda(mean, var)
+    if running_mean is not None:
+        weights_written()
     C = mean.numel()
     scale = torch.empty(C, dtype=torch.float32, device=mean.device)
     shift = torch.empty(C, dtype=torch.float32, device=mean.device)
@@ -862,6 +880,7 @@ def ce_loss(logits, target, class_weight=None, ignore_index=-100, need_grad=True
 def clamp_adam_(param, grad, exp_avg, exp_avg_sq, step, lr, beta1=0.9, beta2=0.999, eps=1e-8,
                 weight_decay=0.0, grad_clip=0.0, grad_scale=1.0):
     _need_cuda(param, grad, exp_avg, exp_avg_sq)
+    weights_written()
     _lib.call("spg_clamp_adam", param, grad, exp_avg, exp_avg_sq, param.numel(), float(lr),
               float(beta1), float(beta2), float(eps), float(weight_decay), float(grad_clip),
               float(grad_scale), int(step), _lib.current_stream())
@@ -871,6 +890,7 @@ def clamp_adam_dev_(param, grad, exp_avg, exp_avg_sq, step_counter, lr, beta1=0.
                     eps=1e-8, weight_decay=0.0, grad_clip=0.0, grad_scale=1.0):
     """clamp + Adam with the step count in device memory (int64 scalar tensor, incremented here)."""
     _need_cuda(param, grad, exp_avg, exp_avg_sq, step_counter)
+    weights_written()
     _lib.call("spg_clamp_adam_dev", param, grad, exp_avg, exp_avg_sq, param.numel(), float(lr),
               float(beta1), float(beta2), float(eps), float(weight_decay), float(grad_clip),
               float(grad_scale), step_counter, _lib.current_stream())
@@ -905,6 +925,7 @@ class FusedAllreduce(object):
     def step_(self, param, exp_avg, exp_avg_sq, step_counter, lr, beta1=0.9, beta2=0.999, eps=1e-8,
               weight_decay=0.0, grad_clip=0.0):
         _need_cuda(param, exp_avg, exp_avg_sq, step_counter)
+        weights_written()
         _lib.call("spg_allreduce_clamp_adam", self.grad, self.stage_ptrs, self.flag_ptrs, self.rank, self.world,
                   param, exp_avg, exp_avg_sq, param.numel(), float(lr), float(beta1), float(beta2), float(eps),
                   float(weight_decay), float(grad_clip), 1.0 / self.world, step_counter, self.state,
@@ -1058,63 +1079,119 @@ def pointnet_fused_supported(F, L, widths):
     return USE_FUSED_EVAL[0] and bool(_lib.lib().spg_pointnet_fused_supported(int(F), int(L), len(widths), w.data_ptr()))
 
 
-_FUSED_IMAGES = {}  # parameter versions -> (weight image, folded bias, widths tensor)
 EVAL_BF16 = [False]  # eval-mode PointNet trunk in bf16 arithmetic (Trainer(dtype="bf16") sets it around eval_step)
+_FUSED_IMAGES = {}  # (F, bf16, ids of the source tensors) -> _FusedImage
+FUSED_RECORD = [None]  # a list while Trainer.capture_eval records the images its graph reads
+
+
+def _fused_sources(layers):
+    """The tensors a folded image is computed from: per layer W, bias, running mean and variance, gamma, beta
+    (None where absent)."""
+    out = []
+    for W, b, bn in layers:
+        out += [W, b] + ([bn.running_mean, bn.running_var, bn.weight, bn.bias] if bn is not None else [None] * 4)
+    return out
+
+
+class _FusedImage(object):
+    """One folded chain: the weight image, the folded bias and the widths, plus what decides whether they still
+    match their sources.  The sources are held by weak reference: an entry never keeps a model alive, and a new
+    tensor that happens to get a freed one's id or address is not mistaken for it.  The stamp is the weights
+    generation and every source's (address, version): torch's in-place operations bump the versions, the
+    library's raw-pointer writers the generation.  A stale entry is refolded in place, so that a captured eval
+    graph, which holds the image's and bias's addresses, reads the refreshed values."""
+
+    def __init__(self, layers, F, bf16):
+        self.F, self.bf16 = int(F), bool(bf16)
+        self.refs = [None if t is None else weakref.ref(t) for t in _fused_sources(layers)]
+        self.bn_refs = [None if bn is None else weakref.ref(bn) for _, _, bn in layers]
+        self.shapes = [tuple(W.shape) for W, _, _ in layers]
+        dev = layers[0][0].device
+        L = _lib.lib()
+        self.widths = torch.tensor([int(W.shape[0]) for W, _, _ in layers], dtype=torch.int32)
+        if bf16:
+            rows = int(L.spg_pointnet_fused_bf16_image_rows(self.F, len(layers), self.widths.data_ptr()))
+            self.image = torch.empty(rows * 64, dtype=torch.bfloat16, device=dev)
+        else:
+            rows = int(L.spg_pointnet_fused_image_rows(self.F, len(layers), self.widths.data_ptr()))
+            self.image = torch.empty(rows * 32, dtype=torch.float32, device=dev)
+        self.bias = torch.empty(int(self.widths.sum()), dtype=torch.float32, device=dev)
+        self._fold(layers)
+
+    def same_sources(self, layers):
+        srcs = _fused_sources(layers)
+        return (len(srcs) == len(self.refs) and [tuple(W.shape) for W, _, _ in layers] == self.shapes
+                and all((r is None and t is None) or (r is not None and r() is t) for r, t in zip(self.refs, srcs)))
+
+    @staticmethod
+    def _stamp(layers):
+        return (WEIGHTS_GENERATION[0],) + tuple(None if t is None else (t.data_ptr(), t._version)
+                                                for t in _fused_sources(layers))
+
+    def refresh(self, layers=None):
+        """Refolds in place if a source changed since the last fold; layers=None: the entry's own sources
+        (nothing to do once they are gone)."""
+        if layers is None:
+            layers = []
+            for i, bnr in enumerate(self.bn_refs):
+                W, b = (None if r is None else r() for r in self.refs[6 * i:6 * i + 2])
+                bn = None if bnr is None else bnr()
+                if W is None or (self.refs[6 * i + 1] is not None and b is None) or (bnr is not None and bn is None):
+                    return
+                layers.append((W, b, bn))
+            if not self.same_sources(layers):
+                return
+        if self._stamp(layers) != self.stamp:
+            self._fold(layers)
+
+    def _fold(self, layers):
+        self.stamp = self._stamp(layers)
+        image, bias, bf16 = self.image, self.bias, self.bf16
+        kc = 64 if bf16 else 32
+        row, boff, K = 0, 0, kc
+        for W, b, bn in layers:
+            N, kv = int(W.shape[0]), int(W.shape[1])
+            scale = shift = None
+            if bn is not None:
+                scale, shift = bn_fold(bn.running_mean, bn.running_var, bn.weight, bn.bias, bn.eps)
+            if bf16:
+                _lib.call("spg_tc_pack_weights_bf16", W, W.stride(0), scale, N, K, kv, image[row * 64:],
+                          _lib.current_stream())
+                row += (K // 64) * N
+            else:
+                _lib.call("spg_tc_pack_weights_scaled", W, W.stride(0), scale, N, K, kv, image[row * 32:],
+                          _lib.current_stream())
+                row += (K // 32) * 2 * N
+            bsl = bias[boff:boff + N]
+            if b is not None:
+                affine_act(b.detach().reshape(1, N), N, 1, N, scale, shift, False, out=bsl, ldo=N)
+            elif shift is not None:
+                bsl.copy_(shift)
+            else:
+                zero_(bsl)
+            boff += N
+            K = max(N, kc) if bf16 else N
 
 
 def pointnet_fused_image(layers, F, bf16=False):
-    """layers: [(W [N,K] (2-D view), bias|None, bn_module|None)] of a Conv1d(k=1)+BatchNorm+ReLU chain in eval
-    mode.  Returns (image, bias, widths): BatchNorm folded into weights and bias (scale = gamma/sqrt(rv+eps),
-    bias' = bias*scale + beta - rm*scale), packed for spg_pointnet_fused_eval (fp32: tf32 hi|lo blocks of 32
-    floats) or spg_pointnet_fused_eval_bf16 (bf16 blocks of 64 elements).  Cached on the tensors' version
-    counters (eval weights do not change between batches)."""
-    key = []
-    for W, b, bn in layers:
-        ts = [W, b] + ([bn.running_mean, bn.running_var, bn.weight, bn.bias] if bn is not None else [])
-        key += [(x.data_ptr(), x._version) for x in ts if x is not None]
-    key = (int(F), bool(bf16)) + tuple(key)
+    """layers: [(W [N,K] or Conv1d weight [N,K,1], bias|None, bn_module|None)] of a Conv1d(k=1)+BatchNorm+ReLU
+    chain in eval mode.  Returns (image, bias, widths): BatchNorm folded into weights and bias
+    (scale = gamma/sqrt(rv+eps), bias' = bias*scale + beta - rm*scale), packed for spg_pointnet_fused_eval
+    (fp32: tf32 hi|lo blocks of 32 floats) or spg_pointnet_fused_eval_bf16 (bf16 blocks of 64 elements).
+    Cached per source tensors (see _FusedImage): pass the same tensor objects on every call (the module's
+    parameters, not fresh views of them), and the image is refolded only when they have changed."""
+    key = (int(F), bool(bf16)) + tuple(None if t is None else id(t) for t in _fused_sources(layers))
     ent = _FUSED_IMAGES.get(key)
-    if ent is not None:
-        return ent
-    dev = layers[0][0].device
-    L = _lib.lib()
-    widths = torch.tensor([int(W.shape[0]) for W, _, _ in layers], dtype=torch.int32)
-    if bf16:
-        rows = int(L.spg_pointnet_fused_bf16_image_rows(int(F), len(layers), widths.data_ptr()))
-        image = torch.empty(rows * 64, dtype=torch.bfloat16, device=dev)
-        kc = 64
+    if ent is None or not ent.same_sources(layers):
+        ent = _FusedImage(layers, F, bf16)
+        if len(_FUSED_IMAGES) > 64:
+            _FUSED_IMAGES.clear()
+        _FUSED_IMAGES[key] = ent
     else:
-        rows = int(L.spg_pointnet_fused_image_rows(int(F), len(layers), widths.data_ptr()))
-        image = torch.empty(rows * 32, dtype=torch.float32, device=dev)
-        kc = 32
-    bias = torch.empty(int(widths.sum()), dtype=torch.float32, device=dev)
-    row, boff, K = 0, 0, kc
-    for W, b, bn in layers:
-        N, kv = int(W.shape[0]), int(W.shape[1])
-        scale = shift = None
-        if bn is not None:
-            scale, shift = bn_fold(bn.running_mean, bn.running_var, bn.weight, bn.bias, bn.eps)
-        if bf16:
-            _lib.call("spg_tc_pack_weights_bf16", W, W.stride(0), scale, N, K, kv, image[row * 64:],
-                      _lib.current_stream())
-            row += (K // 64) * N
-        else:
-            _lib.call("spg_tc_pack_weights_scaled", W, W.stride(0), scale, N, K, kv, image[row * 32:],
-                      _lib.current_stream())
-            row += (K // 32) * 2 * N
-        bsl = bias[boff:boff + N]
-        if b is not None:
-            affine_act(b.detach().reshape(1, N), N, 1, N, scale, shift, False, out=bsl, ldo=N)
-        elif shift is not None:
-            bsl.copy_(shift)
-        else:
-            zero_(bsl)
-        boff += N
-        K = max(N, kc) if bf16 else N
-    if len(_FUSED_IMAGES) > 64:
-        _FUSED_IMAGES.clear()
-    _FUSED_IMAGES[key] = (image, bias, widths)
-    return image, bias, widths
+        ent.refresh(layers)
+    if FUSED_RECORD[0] is not None:
+        FUSED_RECORD[0].append(ent)
+    return ent.image, ent.bias, ent.widths
 
 
 def pointnet_fused_eval(clouds, T, image, bias, widths, pooled, ldp):

@@ -12,7 +12,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .dense import Deferred, _w2d, chain_backward, chain_forward, parse_sequential
+from .dense import Deferred, chain_backward, chain_forward, parse_sequential
 
 
 def _norm_relu(norm, w, n_group):
@@ -172,12 +172,13 @@ class _Segments(_Layout):
 
 
 def _conv_layers(specs, params):
-    """[(W2d, bias, bn)] of a parsed Conv1d(k=1)+BatchNorm+ReLU chain, or None if it is not of that form."""
+    """[(W [N,K,1], bias, bn)] of a parsed Conv1d(k=1)+BatchNorm+ReLU chain, or None if it is not of that form.
+    The parameters themselves, not views of them: ops.pointnet_fused_image caches on the tensors' identity."""
     out = []
     for sp in specs:
         if sp.bn is None or not sp.relu or not sp.bn.track_running_stats or sp.bn.running_mean is None:
             return None
-        out.append((_w2d(params[sp.w]), params[sp.b] if sp.b is not None else None, sp.bn))
+        out.append((params[sp.w], params[sp.b] if sp.b is not None else None, sp.bn))
     return out
 
 

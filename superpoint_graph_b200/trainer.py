@@ -136,6 +136,7 @@ class Trainer(object):
         self.side_in_eager = False  # tests: exercise the two-stream schedule without a graph
         self.step_dev = torch.zeros((), dtype=torch.int64, device=self.flat.device)
         self._graphs = {}
+        self._eval_images = {}  # eval graph key -> the folded PointNet images its graph reads (kept alive here)
         self.class_weights = class_weights
         self.pg, self.world_size = process_group, world_size
         self._fused_ar = None
@@ -297,6 +298,7 @@ class Trainer(object):
     def replay(self, key):
         g, db, loss, logits = self._graphs[key]
         g.replay()
+        ops.weights_written()  # the graph's BatchNorm folds updated the running statistics
         self.apply_update()  # (NCCL path: outside the graph; fused path: one more kernel launch)
         return loss, logits
 
@@ -322,16 +324,24 @@ class Trainer(object):
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         self._capturing = True
+        ops.FUSED_RECORD[0] = images = []
         try:
             with torch.cuda.graph(g):
                 logits = self.eval_step(db)
         finally:
             self._capturing = False
+            ops.FUSED_RECORD[0] = None
         self._graphs[key] = (g, db, None, logits)
+        self._eval_images[key] = images
         return key
 
     def replay_eval(self, key):
+        """Replays a captured inference forward.  The graph reads folded PointNet weight images at fixed
+        addresses: any of them that the weights or running statistics have left behind since (a training step
+        in between) is refolded in place first; with nothing changed, no kernel runs besides the graph."""
         g, db, _, logits = self._graphs[key]
+        for ent in self._eval_images[key]:
+            ent.refresh()
         g.replay()
         return logits
 
