@@ -748,6 +748,54 @@ int spg_knn_query(int64_t n, int k, int k1, double ox, double oy, double oz, dou
 int spg_geof(const float* xyz, int64_t n, const int64_t* target, int k, float* geof, uint32_t* status,
              spg_stream_t stream);
 
+/* ---------------------------------------------------------------- superpoint graph
+ * compute_sp_graph of the partition pipelines (ref: partition/graphs.py:75-210), xyz float32 [n, 3] and
+ * in_component int64 [n] on the device, n < 2^31 - 1.
+ *
+ * spg_sp_scan: words [2] (device, int64) = max(in_component) + 1 (n_com) and a status (1: a non-finite
+ * coordinate, 4: a negative id).
+ * spg_sp_points (workspace: spg_sp_points_workspace bytes, 256-byte aligned; 1 <= n_com <= n): the points sorted
+ * by (component, x, y, z) (-0 == +0), the unique rows of every component (ref: graphs.py:155 np.unique(axis=0));
+ * centroids [n_com, 3] = numpy's mean of them (sequential fp32 sum in sorted order / u), the unique row itself
+ * when u == 1; length, surface, volume [n_com] (float32) = 0 (u == 1), numpy's fp32 sqrt(sum(var)), 0, 0
+ * (u == 2), ev0, sqrt(ev0 ev1 + 1e-10), sqrt(ev0 ev1 ev2 + 1e-10) of the fp64 covariance (ddof 1) in fp64
+ * (u >= 3); point_count [n_com] (int64); sp_labels [n_com, n_label_cols] (int64) = label_mode 1: the histogram of
+ * labels [n] over 0..n_labels (n_label_cols = n_labels + 1; other values not counted), 2: the sum of the rows of
+ * labels [n, n_label_cols]; 0: none (labels and sp_labels may be NULL).  status [1] (device, uint32) = 8 where a
+ * component below n_com holds no point.  ref: graphs.py:146-181
+ * spg_sp_edges_count (workspace: spg_sp_edges_workspace(n_tets, 0) bytes): simplices [n_tets, 4] (int64 when
+ * ids64, else int32); tet_offsets [n_tets + 1] (device, int32) = the exclusive scan of the directed vertex pairs of
+ * every tetrahedron whose endpoints lie in different components, tet_offsets[n_tets] = n_cand, their total; status
+ * [1] = 2 where an id is outside [0, n).  n_tets <= (2^31 - 2) / 12.  ref: graphs.py:86-106
+ * spg_sp_edges_build (workspace: spg_sp_edges_workspace(n_tets, n_cand) bytes): the pairs deduplicated (ref:
+ * graphs.py:108), those with float32 sqrt((dx dx + dy dy) + dz dz) < float32(d_max) kept when d_max > 0 (:110-112),
+ * grouped by the exact 64-bit (source component, target component) key, ascending (:114-124); n_sedg [1] (device,
+ * int64) = the number of superedges.
+ * spg_sp_edges_features (the build's workspace, n_sedg read back): source, target [n_sedg] (int64);
+ * delta_mean, delta_std (ddof 0) [n_sedg, 3] and delta_norm [n_sedg] of delta = xyz[u] - xyz[v] over the pairs, in
+ * fp64 rounded once (one pair: its float32 delta, 0, its float32 norm); delta_centroid [n_sedg, 3] = fp32
+ * centroid difference; length / surface / volume ratios = fp32 a / (b + 1e-6f); point_count_ratio =
+ * float32(double(cs) / (double(ct) + 1e-6)).  ref: graphs.py:183-209                                         */
+int spg_sp_scan(const float* xyz, const int64_t* in_component, int64_t n, int64_t* words, spg_stream_t stream);
+int spg_sp_points_workspace(int64_t n, int64_t* bytes);
+int spg_sp_points(const float* xyz, const int64_t* in_component, int64_t n, int64_t n_com, const int64_t* labels,
+                  int label_mode, int64_t n_label_cols, int n_labels, void* workspace, int64_t workspace_bytes,
+                  float* centroids, float* length, float* surface, float* volume, int64_t* point_count,
+                  int64_t* sp_labels, uint32_t* status, spg_stream_t stream);
+int spg_sp_edges_workspace(int64_t n_tets, int64_t n_cand, int64_t* bytes);
+int spg_sp_edges_count(const int64_t* in_component, int64_t n, const void* simplices, int ids64, int64_t n_tets,
+                       int32_t* tet_offsets, void* workspace, int64_t workspace_bytes, uint32_t* status,
+                       spg_stream_t stream);
+int spg_sp_edges_build(const float* xyz, const int64_t* in_component, int64_t n, const void* simplices, int ids64,
+                       int64_t n_tets, const int32_t* tet_offsets, int64_t n_cand, double d_max, void* workspace,
+                       int64_t workspace_bytes, int64_t* n_sedg, spg_stream_t stream);
+int spg_sp_edges_features(const float* xyz, int64_t n_tets, int64_t n_cand, const void* workspace,
+                          int64_t workspace_bytes, int64_t n_sedg, const float* centroids, const float* length,
+                          const float* surface, const float* volume, const int64_t* point_count, int64_t* source,
+                          int64_t* target, float* delta_mean, float* delta_std, float* delta_norm,
+                          float* delta_centroid, float* length_ratio, float* surface_ratio, float* volume_ratio,
+                          float* point_count_ratio, spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

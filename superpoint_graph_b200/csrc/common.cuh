@@ -83,6 +83,12 @@ enum KernelId {
     K_GEO_GRID,
     K_GEO_KNN,
     K_GEO_GEOF,
+    K_SP_SCAN,
+    K_SP_SORT_KEYS,
+    K_SP_POINTS,
+    K_SP_TETS,
+    K_SP_PAIRS,
+    K_SP_EDGES,
     K_COUNT
 };
 

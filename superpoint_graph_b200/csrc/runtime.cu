@@ -31,6 +31,8 @@ static const char* kKernelNames[K_COUNT] = {
     "lp_weights",        "lp_relax",           "lp_metrics",
     "lp_augment",        "lp_subgraph",        "lp_local_clouds",
     "geo_bounds",        "geo_grid",           "geo_knn",             "geo_geof",
+    "sp_scan",           "sp_sort_keys",       "sp_points",           "sp_tets",
+    "sp_pairs",          "sp_edges",
 };
 
 struct Record {

@@ -1473,3 +1473,92 @@ def geof(xyz, target, k):
     status = torch.empty(1, dtype=torch.int32, device=xyz.device)
     _lib.call("spg_geof", xyz, n, target, int(k), out, status, _lib.current_stream())
     return out, status
+
+
+# ------------------------------------------------------------- superpoint graph
+def sp_scan(xyz, in_component):
+    """int64 [2] on the device: max(in_component) + 1 and the status word (1: a non-finite coordinate, 4: a negative
+    id); see spg_sp_scan."""
+    _need_cuda(xyz, in_component)
+    assert xyz.dtype == torch.float32 and xyz.is_contiguous()
+    assert in_component.dtype == torch.int64 and in_component.is_contiguous()
+    words = torch.empty(2, dtype=torch.int64, device=xyz.device)
+    _lib.call("spg_sp_scan", xyz, in_component, xyz.shape[0], words, _lib.current_stream())
+    return words
+
+
+def sp_points(xyz, in_component, n_com, labels, label_mode, n_labels):
+    """The superpoint features (centroids [n_com, 3], length, surface, volume [n_com, 1] float32, point_count
+    [n_com, 1] int64, sp_labels [n_com, n_label_cols] int64 or None) and the status word (int32 [1]; 8: an empty
+    component); see spg_sp_points.  labels: None, int64 [n] (label_mode 1) or int64 [n, L] (label_mode 2)."""
+    _need_cuda(xyz, in_component, labels)
+    assert in_component.dtype == torch.int64 and in_component.is_contiguous()
+    dev, n = xyz.device, xyz.shape[0]
+    nbytes = torch.zeros(1, dtype=torch.int64)
+    _lib.call("spg_sp_points_workspace", int(n), nbytes)
+    ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=dev)
+    cols = 0
+    if label_mode:
+        assert labels.dtype == torch.int64 and labels.is_contiguous()
+        cols = n_labels + 1 if label_mode == 1 else labels.shape[1]
+    cen = torch.empty((n_com, 3), dtype=torch.float32, device=dev)
+    f = [torch.empty((n_com, 1), dtype=torch.float32, device=dev) for _ in range(3)]
+    count = torch.empty((n_com, 1), dtype=torch.int64, device=dev)
+    sp_labels = torch.empty((n_com, cols), dtype=torch.int64, device=dev) if label_mode else None
+    status = torch.empty(1, dtype=torch.int32, device=dev)
+    _lib.call("spg_sp_points", xyz, in_component, int(n), int(n_com), labels, int(label_mode), int(cols),
+              int(n_labels), ws, ws.numel(), cen, f[0], f[1], f[2], count, sp_labels, status, _lib.current_stream())
+    return (cen, f[0], f[1], f[2], count, sp_labels), status
+
+
+def _edges_workspace(n_tets, n_cand, device):
+    nbytes = torch.zeros(1, dtype=torch.int64)
+    _lib.call("spg_sp_edges_workspace", int(n_tets), int(n_cand), nbytes)
+    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
+
+
+def sp_edges_count(in_component, simplices):
+    """(tet_offsets int32 [T + 1], status int32 [1]; 2: an id outside [0, n)) on the device for simplices int32 or
+    int64 [T, 4]; tet_offsets[T] is the number of candidate pairs.  See spg_sp_edges_count."""
+    _need_cuda(in_component, simplices)
+    assert simplices.dtype in (torch.int32, torch.int64) and simplices.is_contiguous()
+    dev, t = in_component.device, simplices.shape[0]
+    ws = _edges_workspace(t, 0, dev)
+    offsets = torch.empty(t + 1, dtype=torch.int32, device=dev)
+    status = torch.empty(1, dtype=torch.int32, device=dev)
+    _lib.call("spg_sp_edges_count", in_component, in_component.shape[0], simplices,
+              int(simplices.dtype == torch.int64), int(t), offsets, ws, ws.numel(), status, _lib.current_stream())
+    return offsets, status
+
+
+def sp_edges_build(xyz, in_component, simplices, offsets, n_cand, d_max):
+    """(workspace, n_sedg int64 [1] on the device): the superedges' pairs grouped by component key; see
+    spg_sp_edges_build."""
+    _need_cuda(xyz, in_component, simplices, offsets)
+    dev, t = xyz.device, simplices.shape[0]
+    ws = _edges_workspace(t, n_cand, dev)
+    n_sedg = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.call("spg_sp_edges_build", xyz, in_component, xyz.shape[0], simplices, int(simplices.dtype == torch.int64),
+              int(t), offsets, int(n_cand), float(d_max), ws, ws.numel(), n_sedg, _lib.current_stream())
+    return ws, n_sedg
+
+
+def sp_edges_features(xyz, n_tets, n_cand, ws, n_sedg, sp):
+    """dict of source, target [n_sedg, 1] (int64) and the se_* features (float32); see spg_sp_edges_features.
+    sp = (centroids, length, surface, volume, point_count) from sp_points."""
+    _need_cuda(xyz, ws, *sp)
+    dev = xyz.device
+    src = torch.empty((n_sedg, 1), dtype=torch.int64, device=dev)
+    tgt = torch.empty((n_sedg, 1), dtype=torch.int64, device=dev)
+    f3 = {k: torch.empty((n_sedg, 3), dtype=torch.float32, device=dev)
+          for k in ("se_delta_mean", "se_delta_std", "se_delta_centroid")}
+    f1 = {k: torch.empty((n_sedg, 1), dtype=torch.float32, device=dev)
+          for k in ("se_delta_norm", "se_length_ratio", "se_surface_ratio", "se_volume_ratio", "se_point_count_ratio")}
+    _lib.call("spg_sp_edges_features", xyz, int(n_tets), int(n_cand), ws, ws.numel(), int(n_sedg), *sp, src, tgt,
+              f3["se_delta_mean"], f3["se_delta_std"], f1["se_delta_norm"], f3["se_delta_centroid"],
+              f1["se_length_ratio"], f1["se_surface_ratio"], f1["se_volume_ratio"], f1["se_point_count_ratio"],
+              _lib.current_stream())
+    out = {"source": src, "target": tgt}
+    out.update(f3)
+    out.update(f1)
+    return out
