@@ -796,6 +796,37 @@ int spg_sp_edges_features(const float* xyz, int64_t n_tets, int64_t n_cand, cons
                           float* delta_centroid, float* length_ratio, float* surface_ratio, float* volume_ratio,
                           float* point_count_ratio, spg_stream_t stream);
 
+/* ---------------------------------------------------------------- voxel pruning
+ * prune of the partition pipelines (ref: partition/ply_c/ply_c.cpp:149-380; called at partition/partition.py:124,
+ * supervized_partition/graph_processing.py:124,142 and, chunk by chunk, partition/provider.py:250-303), xyz float32
+ * [n, 3] on the device, 1 <= n < 2^31 - 1.  chunk_rows = 0: one cloud; > 0: every chunk of chunk_rows consecutive
+ * points is pruned on its own (its own minimum) and the voxels are stacked in chunk order.  One workspace of
+ * spg_prune_workspace(n, chunk_rows) bytes (256-byte aligned) serves the three calls, in order.
+ *
+ * spg_prune_bounds: words [4] (device, int64) = status (1: a non-finite coordinate, 2: a bin of 2^32 or more, 4: a
+ * label outside [0, n_labels], 8: an object outside [0, n_objects]) and the largest bin of x, y and z over the
+ * chunks.  A bin is (uint32) floor((x - x_min) / voxel_size) in fp32, x_min the chunk's minimum.  labels and objects
+ * (int64 [n]) are read only where the reference reads them: labels when n_labels > 0, objects when n_labels > 0 and
+ * n_objects > 0.  ref: ply_c.cpp:305-331
+ * spg_prune_voxels (max_bin_* from the bounds): the points stably sorted by (chunk, bin x, bin y, bin z), packed into
+ * the fewest bits that hold them (two sorts beyond 64 bits); the voxels numbered in order of first touch in point
+ * order (the reference's insertion order); n_voxels [1] (device, int64) = m.  ref: ply_c.cpp:326-336
+ * spg_prune_reduce (m read back): xyz_out [m, 3] = the fp32 sum of the voxel's points in point order from 0.f /
+ * (float) count; rgb_out [m, 3] (uint8) = (uint8)((float) uint32 sum / (float) count); labels_out [m, n_labels + 1]
+ * and objects_out [m, n_objects + 1] (int64) = the histograms, zero where the reference counts nothing.
+ * ref: ply_c.cpp:338-379                                                                                   */
+int spg_prune_workspace(int64_t n, int64_t chunk_rows, int64_t* bytes);
+int spg_prune_bounds(const float* xyz, int64_t n, int64_t chunk_rows, float voxel_size, const int64_t* labels,
+                     int n_labels, const int64_t* objects, int n_objects, void* workspace, int64_t workspace_bytes,
+                     int64_t* words, spg_stream_t stream);
+int spg_prune_voxels(const float* xyz, int64_t n, int64_t chunk_rows, float voxel_size, int64_t max_bin_x,
+                     int64_t max_bin_y, int64_t max_bin_z, void* workspace, int64_t workspace_bytes,
+                     int64_t* n_voxels, spg_stream_t stream);
+int spg_prune_reduce(const float* xyz, const uint8_t* rgb, const int64_t* labels, int n_labels,
+                     const int64_t* objects, int n_objects, int64_t n, int64_t chunk_rows, const void* workspace,
+                     int64_t workspace_bytes, int64_t n_voxels, float* xyz_out, uint8_t* rgb_out,
+                     int64_t* labels_out, int64_t* objects_out, spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,7 +3,10 @@
     python -m superpoint_graph_b200.build [--force]
 
 Objects go to build/ (git-ignored); the shared library lands next to this file so that it
-travels with the repository snapshot to the GPU box.
+travels with the repository snapshot to the GPU box.  With SPG_REFERENCE set to a reference
+checkout, the recipe oracle/build_ref.py also compiles the reference's own `prune` into
+oracle/_ref/ (git-ignored) for the tests to compare against; it runs as a separate process,
+so the product never imports the oracle.
 """
 import os
 import shutil
@@ -66,7 +69,20 @@ def build(force=False, verbose=True):
         if verbose:
             print("[spg build]", " ".join(cmd), flush=True)
         subprocess.check_call(cmd)
+    _build_reference(force, verbose)
     return LIB_PATH
+
+
+def _build_reference(force, verbose):
+    if not os.environ.get("SPG_REFERENCE"):
+        return
+    recipe = os.path.join(ROOT, "oracle", "build_ref.py")
+    out = os.path.join(ROOT, "oracle", "_ref", "libply_c_prune.so")
+    if not force and os.path.exists(out) and os.path.getmtime(out) >= os.path.getmtime(recipe):
+        return
+    if verbose:
+        print("[spg build]", sys.executable, recipe, flush=True)
+    subprocess.check_call([sys.executable, recipe])
 
 
 if __name__ == "__main__":

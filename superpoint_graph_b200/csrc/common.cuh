@@ -89,6 +89,10 @@ enum KernelId {
     K_SP_TETS,
     K_SP_PAIRS,
     K_SP_EDGES,
+    K_PRUNE_BOUNDS,
+    K_PRUNE_KEYS,
+    K_PRUNE_ROWS,
+    K_PRUNE_REDUCE,
     K_COUNT
 };
 

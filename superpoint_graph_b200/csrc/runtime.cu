@@ -33,6 +33,7 @@ static const char* kKernelNames[K_COUNT] = {
     "geo_bounds",        "geo_grid",           "geo_knn",             "geo_geof",
     "sp_scan",           "sp_sort_keys",       "sp_points",           "sp_tets",
     "sp_pairs",          "sp_edges",
+    "prune_bounds",      "prune_keys",         "prune_rows",          "prune_reduce",
 };
 
 struct Record {

@@ -1562,3 +1562,49 @@ def sp_edges_features(xyz, n_tets, n_cand, ws, n_sedg, sp):
     out.update(f3)
     out.update(f1)
     return out
+
+
+# ------------------------------------------------------------- voxel pruning
+def prune_workspace(n, chunk_rows, device):
+    nbytes = torch.zeros(1, dtype=torch.int64)
+    _lib.call("spg_prune_workspace", int(n), int(chunk_rows), nbytes)
+    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
+
+
+def prune_bounds(xyz, chunk_rows, voxel_size, labels, n_labels, objects, n_objects, ws):
+    """int64 [4] on the device: the status word (1: a non-finite coordinate, 2: a bin >= 2^32, 4: a label outside
+    [0, n_labels], 8: an object outside [0, n_objects]) and the largest bin of x, y, z; see spg_prune_bounds."""
+    _need_cuda(xyz, labels, objects, ws)
+    assert xyz.dtype == torch.float32 and xyz.is_contiguous()
+    for t in (labels, objects):
+        assert t is None or (t.dtype == torch.int64 and t.is_contiguous())
+    words = torch.empty(4, dtype=torch.int64, device=xyz.device)
+    _lib.call("spg_prune_bounds", xyz, xyz.shape[0], int(chunk_rows), float(voxel_size), labels, int(n_labels),
+              objects, int(n_objects), ws, ws.numel(), words, _lib.current_stream())
+    return words
+
+
+def prune_voxels(xyz, chunk_rows, voxel_size, max_bins, ws):
+    """int64 [1] on the device: the number of voxels; the sorted points and the voxels' runs stay in `ws`.  See
+    spg_prune_voxels."""
+    _need_cuda(xyz, ws)
+    n_voxels = torch.empty(1, dtype=torch.int64, device=xyz.device)
+    _lib.call("spg_prune_voxels", xyz, xyz.shape[0], int(chunk_rows), float(voxel_size), int(max_bins[0]),
+              int(max_bins[1]), int(max_bins[2]), ws, ws.numel(), n_voxels, _lib.current_stream())
+    return n_voxels
+
+
+def prune_reduce(xyz, rgb, labels, n_labels, objects, n_objects, chunk_rows, ws, m):
+    """(xyz [m, 3] float32, rgb [m, 3] uint8, labels [m, n_labels + 1] int64, objects [m, n_objects + 1] int64) of
+    the m voxels that prune_voxels left in `ws`; see spg_prune_reduce."""
+    _need_cuda(xyz, rgb, labels, objects, ws)
+    assert rgb.dtype == torch.uint8 and rgb.is_contiguous()
+    dev = xyz.device
+    xyz_out = torch.empty((m, 3), dtype=torch.float32, device=dev)
+    rgb_out = torch.empty((m, 3), dtype=torch.uint8, device=dev)
+    labels_out = torch.empty((m, n_labels + 1), dtype=torch.int64, device=dev)
+    objects_out = torch.empty((m, n_objects + 1), dtype=torch.int64, device=dev)
+    _lib.call("spg_prune_reduce", xyz, rgb, labels, int(n_labels), objects, int(n_objects), xyz.shape[0],
+              int(chunk_rows), ws, ws.numel(), int(m), xyz_out, rgb_out, labels_out, objects_out,
+              _lib.current_stream())
+    return xyz_out, rgb_out, labels_out, objects_out
