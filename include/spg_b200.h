@@ -13,6 +13,10 @@
  * kernels only; it exists for gradcheck-style tests, reference
  * learning/ecc/test_GraphConvModule.py:25).
  *
+ * A call whose scratch is sized by a `spg_*_workspace` query takes that scratch as one `workspace`
+ * argument and no other: 256-byte aligned (else SPG_E_ALIGN) and at least the reported bytes (else
+ * SPG_E_BADARG), both checked before any kernel is launched.  The reported size is exact, with no slack.
+ *
  * Each function names the reference code it replaces as
  * `ref: <file>:<lines>` relative to the reference repository root.
  */
@@ -590,16 +594,16 @@ int spg_nn1_interpolate(const float* xyz_ref, int64_t n_ref, const float* xyz_qu
  * Edge arrays src/tgt are int64 [E] device arrays; is_transition is uint8 [E] (0 = intra, 1 = inter);
  * pred_in_component int64 [V].  Endpoints outside [0, V) are skipped (never read).  No float atomics:
  * every float output is bit-reproducible.
- * spg_lp_sort_workspace: bytes of the CUB scratch (`workspace`) of every sorting/scanning call below
- * for up to n items (2E for spg_lp_incidence, max(V, E) for spg_lp_xpart, V for spg_lp_seal).        */
-int spg_lp_sort_workspace(int64_t n, int64_t* bytes);
+ * spg_lp_workspace: bytes of the scratch (`workspace`, 256-byte aligned) of spg_lp_incidence, spg_lp_xpart
+ * and spg_lp_seal for up to n_ver vertices, n_edges edges and n_comp components; a call whose own counts
+ * need more than workspace_bytes returns SPG_E_BADARG.                                                  */
+int spg_lp_workspace(int64_t n_ver, int64_t n_edges, int64_t n_comp, int64_t* bytes);
 /* Per-vertex incidence CSR of the edge endpoints: entry j < E is the source side of edge j, j >= E the
  * target side of edge j - E; rowptr [V+1], entry [2E] sorted by vertex, stably (by j within a vertex).
- * keys_tmp, keys_sorted, vals_tmp: int32 [2E] scratch.  No reference counterpart: the gather CSR of the
- * deterministic backward of compute_dist (ref: supervized_partition/losses.py:31-42 under autograd).  */
+ * No reference counterpart: the gather CSR of the deterministic backward of compute_dist
+ * (ref: supervized_partition/losses.py:31-42 under autograd).                                         */
 int spg_lp_incidence(const int64_t* src, const int64_t* tgt, int64_t n_ver, int64_t n_edges, int32_t* rowptr,
-                     int32_t* entry, int32_t* keys_tmp, int32_t* keys_sorted, int32_t* vals_tmp, void* workspace,
-                     int64_t workspace_bytes, spg_stream_t stream);
+                     int32_t* entry, void* workspace, int64_t workspace_bytes, spg_stream_t stream);
 /* diff[e] from embeddings emb [V, D] (dist_type 0 = euclidian: |x_s - x_t|^2, 1 = intrinsic:
  * (acos(0.999 x_s.x_t) - acos(0.999)) / (acos(-0.999) - acos(0.999)) * 3.141592, 2 = scalar: x_s.x_t - 1),
  * fp64 inside; coef [E] (intrinsic, scalar; may be NULL for euclidian) = d diff / d (x_s.x_t).
@@ -625,23 +629,20 @@ int spg_lp_loss_bwd(const float* diff, const float* weights, const uint8_t* is_t
  * pred_in_component[s] == pred_in_component[t] (components numbered by their smallest vertex:
  * in_component_x [V], comp_size [V] (first n_comp used), n_comp [1]); every transition edge between
  * components (c1, c2) gets 1 + min(|c1|, |c2|) / #(transition edges between c1 and c2) * transition_factor
- * (fp64, rounded once), every other edge 1.  Scratch: parent, is_root, root_rank int32 [V];
- * keys_tmp, keys_sorted uint64 [E]; vals_tmp, vals_sorted int32 [E].
+ * (fp64, rounded once), every other edge 1.
  * ref: supervized_partition/losses.py:130-158 (+ partition/ply_c/connected_components.cpp:17-110, cutoff 0) */
 int spg_lp_xpart(const int64_t* src, const int64_t* tgt, const uint8_t* is_transition,
                  const int64_t* pred_in_component, int64_t n_ver, int64_t n_edges, double transition_factor,
-                 float* weights, int32_t* in_component_x, int32_t* comp_size, int32_t* n_comp, int32_t* parent,
-                 int32_t* is_root, int32_t* root_rank, uint64_t* keys_tmp, uint64_t* keys_sorted, int32_t* vals_tmp,
-                 int32_t* vals_sorted, void* workspace, int64_t workspace_bytes, spg_stream_t stream);
+                 float* weights, int32_t* in_component_x, int32_t* comp_size, int32_t* n_comp, void* workspace,
+                 int64_t workspace_bytes, spg_stream_t stream);
 /* SEAL weights: w[c] = |c| - (frequency of the most common object id in c) for the n_comp predicted
  * components (objects: int64 [V], 0 <= id < 2^32); transition edges get 1 + max(w[c_s], w[c_t]) *
  * transition_factor (fp64, rounded once), others 1; w_per_component [n_comp] (may be NULL).
- * Scratch: size_tmp, maxfreq_tmp int32 [n_comp]; keys_tmp, keys_sorted uint64 [V].
  * ref: supervized_partition/losses.py:119-128,168-173                                                    */
 int spg_lp_seal(const int64_t* src, const int64_t* tgt, const uint8_t* is_transition, const int64_t* pred_in_component,
                 const int64_t* objects, int64_t n_ver, int64_t n_edges, int64_t n_comp, double transition_factor,
-                float* weights, int32_t* w_per_component, int32_t* size_tmp, int32_t* maxfreq_tmp, uint64_t* keys_tmp,
-                uint64_t* keys_sorted, void* workspace, int64_t workspace_bytes, spg_stream_t stream);
+                float* weights, int32_t* w_per_component, void* workspace, int64_t workspace_bytes,
+                spg_stream_t stream);
 /* weights[e] = is_transition[e] != 0 ? w_transition : w_other ('none', 'proportional';
  * ref: supervized_partition/losses.py:96-101)                                                            */
 int spg_lp_fill_weights(const uint8_t* is_transition, int64_t n_edges, float w_other, float w_transition,

@@ -123,6 +123,16 @@ __device__ __forceinline__ void st_stream4(float4* p, float4 v) { __stcs(p, v); 
 
 __device__ __forceinline__ float sigmoidf_(float v) { return 1.f / (1.f + expf(-v)); }
 
+// Order-preserving map float -> uint32 and its inverse: unsigned order of the keys is the order of the floats
+// (-0 below +0), so integer min / max / sorts of keys are min / max / sorts of the floats.
+__device__ __forceinline__ unsigned float_key(float f) {
+    const unsigned u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float float_unkey(unsigned k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
 // ---- BatchNorm/ReLU elements shared by the dense, max-pool and tensor-core kernels
 
 // Gradient through relu(y*sc + sh): g where the pre-activation is > 0, else 0 (NaN included).

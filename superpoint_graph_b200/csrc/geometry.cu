@@ -26,7 +26,7 @@
 // No float atomics anywhere: every output is reproducible bit for bit.
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "workspace.cuh"
 #include "eig3.cuh"
 
 namespace spg {
@@ -37,12 +37,6 @@ constexpr int kKnnMaxK = 64;       // neighbours per query (the vertex itself no
 constexpr int kGridBits = 21;      // per axis
 constexpr double kRingMargin = 1e-6;  // in cells: far above the rounding of a point's cell coordinate (< 2^-30)
 constexpr int kRingColumns = 128;     // (x, y) columns a query visits ring by ring before it sweeps the cell table
-
-// order-preserving map float -> uint32 (min / max over the map are min / max over the floats)
-__device__ __forceinline__ unsigned geo_fkey(float f) {
-    const unsigned u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 // ------------------------------------------------------------------------------------------------ bounds
 // words[0..2] min keys (preset to 0xffffffff), words[3..5] max keys (preset to 0), words[6] status (preset to 0)
@@ -58,7 +52,7 @@ __global__ void __launch_bounds__(GEO_THREADS) geo_bounds_kernel(const float* __
                 bad = 1u;
                 continue;
             }
-            const unsigned k = geo_fkey(v);
+            const unsigned k = float_key(v);
             lo[c] = min(lo[c], k);
             hi[c] = max(hi[c], k);
         }
@@ -373,42 +367,39 @@ __global__ void __launch_bounds__(GEO_THREADS) geo_geof_kernel(const float* __re
 }
 
 // ------------------------------------------------------------------------------------------------ plan
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct KnnWs {
-    size_t keys_in, keys, idx_in, order, sorted_xyz, cell_keys, cell_count, cell_start, n_cells, cub, total;
-    size_t cub_bytes;
+    uint64_t *keys_in, *keys;
+    int32_t *idx_in, *order;
+    float4* sorted_xyz;
+    uint64_t* cell_keys;
+    int32_t *cell_count, *cell_start, *n_cells;
+    CubRegion cub;
+    size_t bytes;
 };
 
-static int plan(int64_t n, KnnWs* w) {
+static int layout(int64_t n, void* base, KnnWs* w) {
     const int m = (int)(n > 0 ? n : 1);
-    size_t a = 0, b = 0, c = 0;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, a, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                                    (const int32_t*)nullptr, (int32_t*)nullptr, m, 0, 3 * kGridBits);
-    if (e != cudaSuccess) return (int)e;
-    e = cub::DeviceRunLengthEncode::Encode(nullptr, b, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                           (int32_t*)nullptr, (int32_t*)nullptr, m);
-    if (e != cudaSuccess) return (int)e;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, c, (const int32_t*)nullptr, (int32_t*)nullptr, m + 1);
-    if (e != cudaSuccess) return (int)e;
-    w->cub_bytes = a > b ? (a > c ? a : c) : (b > c ? b : c);
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (const int32_t*)nullptr, (int32_t*)nullptr, m, 0, 3 * kGridBits);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRunLengthEncode::Encode, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (int32_t*)nullptr, (int32_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::ExclusiveSum, (const int32_t*)nullptr, (int32_t*)nullptr, m + 1);
     const size_t N = (size_t)m;
-    size_t o = 0;
-    w->keys_in = o;     o += align256(N * 8);
-    w->keys = o;        o += align256(N * 8);
-    w->idx_in = o;      o += align256(N * 4);
-    w->order = o;       o += align256(N * 4);
-    w->sorted_xyz = o;  o += align256(N * 16);
-    w->cell_keys = o;   o += align256(N * 8);
-    w->cell_count = o;  o += align256((N + 1) * 4);
-    w->cell_start = o;  o += align256((N + 1) * 4);
-    w->n_cells = o;     o += 256;
-    w->cub = o;         o += align256(w->cub_bytes);
-    w->total = o;
+    Planner p(base);
+    w->keys_in = p.take<uint64_t>(N);
+    w->keys = p.take<uint64_t>(N);
+    w->idx_in = p.take<int32_t>(N);
+    w->order = p.take<int32_t>(N);
+    w->sorted_xyz = p.take<float4>(N);
+    w->cell_keys = p.take<uint64_t>(N);
+    w->cell_count = p.take<int32_t>(N + 1);
+    w->cell_start = p.take<int32_t>(N + 1);
+    w->n_cells = p.take<int32_t>(1);
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
-
-static bool too_big(int64_t n) { return n >= (1ll << 31) - 1; }
 
 static int make_grid(double ox, double oy, double oz, double cell, int64_t dx, int64_t dy, int64_t dz, Grid* g) {
     if (!(cell > 0.0) || !isfinite(cell)) return SPG_E_BADARG;
@@ -436,10 +427,9 @@ int spg_knn_workspace(int64_t n, int64_t* bytes) {
     if (!bytes || n < 0) return SPG_E_BADARG;
     if (too_big(n)) return SPG_E_UNSUPPORTED;
     KnnWs w;
-    const int rc = plan(n, &w);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)w.total;
-    return SPG_OK;
+    const int rc = layout(n, nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_knn_bounds(const float* xyz, int64_t n, uint32_t* words, spg_stream_t stream) {
@@ -458,44 +448,29 @@ int spg_knn_bounds(const float* xyz, int64_t n, uint32_t* words, spg_stream_t st
 int spg_knn_grid(const float* xyz, int64_t n, double ox, double oy, double oz, double cell, int64_t dim_x,
                  int64_t dim_y, int64_t dim_z, void* workspace, int64_t workspace_bytes, int32_t* n_cells,
                  spg_stream_t stream) {
-    if (n <= 0 || !xyz || !workspace || !n_cells) return SPG_E_BADARG;
+    if (n <= 0 || !xyz || !n_cells) return SPG_E_BADARG;
     if (too_big(n)) return SPG_E_UNSUPPORTED;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
-    Grid g;
-    int rc = make_grid(ox, oy, oz, cell, dim_x, dim_y, dim_z, &g);
-    if (rc != SPG_OK) return rc;
     KnnWs w;
-    rc = plan(n, &w);
+    int rc = layout(n, workspace, &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
+    Grid g;
+    rc = make_grid(ox, oy, oz, cell, dim_x, dim_y, dim_z, &g);
+    if (rc != SPG_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    uint64_t* keys_in = reinterpret_cast<uint64_t*>(ws + w.keys_in);
-    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + w.keys);
-    int32_t* idx_in = reinterpret_cast<int32_t*>(ws + w.idx_in);
-    int32_t* order = reinterpret_cast<int32_t*>(ws + w.order);
-    int32_t* cell_count = reinterpret_cast<int32_t*>(ws + w.cell_count);
-    int32_t* nc = reinterpret_cast<int32_t*>(ws + w.n_cells);
     const unsigned blocks = (unsigned)ceil_div64(n, GEO_THREADS);
-    SPG_LAUNCH(K_GEO_GRID, s, geo_keys_kernel, blocks, GEO_THREADS, 0, xyz, n, g, keys_in, idx_in);
-    size_t cb = w.cub_bytes;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(ws + w.cub, cb, (const uint64_t*)keys_in, keys,
-                                                    (const int32_t*)idx_in, order, (int)n, 0, 3 * kGridBits, s);
-    if (e != cudaSuccess) return (int)e;
-    SPG_LAUNCH(K_GEO_GRID, s, geo_gather_kernel, blocks, GEO_THREADS, 0, xyz, n, (const int32_t*)order,
-               reinterpret_cast<float4*>(ws + w.sorted_xyz));
+    SPG_LAUNCH(K_GEO_GRID, s, geo_keys_kernel, blocks, GEO_THREADS, 0, xyz, n, g, w.keys_in, w.idx_in);
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const uint64_t*)w.keys_in, w.keys, (const int32_t*)w.idx_in,
+            w.order, (int)n, 0, 3 * kGridBits, s);
+    SPG_LAUNCH(K_GEO_GRID, s, geo_gather_kernel, blocks, GEO_THREADS, 0, xyz, n, (const int32_t*)w.order,
+               w.sorted_xyz);
     // counts beyond the last cell stay 0, so the scan puts n at cell_start[n_cells] (and after it)
-    e = cudaMemsetAsync(cell_count, 0, ((size_t)n + 1) * 4, s);
+    cudaError_t e = cudaMemsetAsync(w.cell_count, 0, ((size_t)n + 1) * 4, s);
     if (e != cudaSuccess) return (int)e;
-    cb = w.cub_bytes;
-    e = cub::DeviceRunLengthEncode::Encode(ws + w.cub, cb, (const uint64_t*)keys,
-                                           reinterpret_cast<uint64_t*>(ws + w.cell_keys), cell_count, nc, (int)n, s);
-    if (e != cudaSuccess) return (int)e;
-    cb = w.cub_bytes;
-    e = cub::DeviceScan::ExclusiveSum(ws + w.cub, cb, (const int32_t*)cell_count,
-                                      reinterpret_cast<int32_t*>(ws + w.cell_start), (int)n + 1, s);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaMemcpyAsync(n_cells, nc, sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
+    SPG_CUB(w.cub, cub::DeviceRunLengthEncode::Encode, (const uint64_t*)w.keys, w.cell_keys, w.cell_count, w.n_cells,
+            (int)n, s);
+    SPG_CUB(w.cub, cub::DeviceScan::ExclusiveSum, (const int32_t*)w.cell_count, w.cell_start, (int)n + 1, s);
+    e = cudaMemcpyAsync(n_cells, w.n_cells, sizeof(int32_t), cudaMemcpyDeviceToDevice, s);
     if (e != cudaSuccess) return (int)e;
     return launch_status();
 }
@@ -503,27 +478,25 @@ int spg_knn_grid(const float* xyz, int64_t n, double ox, double oy, double oz, d
 int spg_knn_query(int64_t n, int k, int k1, double ox, double oy, double oz, double cell, int64_t dim_x,
                   int64_t dim_y, int64_t dim_z, const void* workspace, int64_t workspace_bytes, int64_t* source,
                   int64_t* target, float* distances, int64_t* target2, spg_stream_t stream) {
-    if (n <= 0 || k <= 0 || k1 <= 0 || k1 > k || !workspace || !source || !target || !distances) return SPG_E_BADARG;
+    if (n <= 0 || k <= 0 || k1 <= 0 || k1 > k || !source || !target || !distances) return SPG_E_BADARG;
     if (k > kKnnMaxK || too_big(n)) return SPG_E_UNSUPPORTED;
     if (n < (int64_t)k + 1) return SPG_E_BADARG;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
-    KnnArgs a;
-    int rc = make_grid(ox, oy, oz, cell, dim_x, dim_y, dim_z, &a.g);
-    if (rc != SPG_OK) return rc;
     KnnWs w;
-    rc = plan(n, &w);
+    int rc = layout(n, const_cast<void*>(workspace), &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
-    const uint8_t* ws = static_cast<const uint8_t*>(workspace);
+    KnnArgs a;
+    rc = make_grid(ox, oy, oz, cell, dim_x, dim_y, dim_z, &a.g);
+    if (rc != SPG_OK) return rc;
     a.n = n;
     a.k = k;
     a.k1 = k1;
-    a.sorted_xyz = reinterpret_cast<const float4*>(ws + w.sorted_xyz);
-    a.order = reinterpret_cast<const int32_t*>(ws + w.order);
-    a.keys = reinterpret_cast<const uint64_t*>(ws + w.keys);
-    a.cell_keys = reinterpret_cast<const uint64_t*>(ws + w.cell_keys);
-    a.cell_start = reinterpret_cast<const int32_t*>(ws + w.cell_start);
-    a.n_cells = reinterpret_cast<const int32_t*>(ws + w.n_cells);
+    a.sorted_xyz = w.sorted_xyz;
+    a.order = w.order;
+    a.keys = w.keys;
+    a.cell_keys = w.cell_keys;
+    a.cell_start = w.cell_start;
+    a.n_cells = w.n_cells;
     a.source = source;
     a.target = target;
     a.distances = distances;

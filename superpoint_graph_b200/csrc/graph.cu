@@ -13,7 +13,7 @@
 // kernels around them are this file's.  Integer work, HBM/latency bound, a few microseconds at batch size.
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "workspace.cuh"
 
 namespace spg {
 
@@ -76,26 +76,23 @@ static int key_bits(int64_t n_in) {
     return b;
 }
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct GraphWs {
-    size_t degs32, iota, keys, cub, total;
-    size_t cub_bytes;
+    int *degs32, *iota, *keys;
+    CubRegion cub;
+    size_t bytes;
 };
 
-static int plan(int64_t n_out, int64_t n_in, int64_t n_edges, GraphWs* w) {
-    size_t scan_b = 0, sort_b = 0;
-    cudaError_t e = cub::DeviceScan::InclusiveSum(nullptr, scan_b, (const int*)nullptr, (int*)nullptr, (int)n_out);
-    if (e != cudaSuccess) return (int)e;
-    e = cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const int*)nullptr, (int*)nullptr, (const int*)nullptr,
-                                        (int*)nullptr, (int)n_edges, 0, key_bits(n_in));
-    if (e != cudaSuccess) return (int)e;
-    w->cub_bytes = scan_b > sort_b ? scan_b : sort_b;
-    w->degs32 = 0;
-    w->iota = w->degs32 + align256((size_t)n_out * 4);
-    w->keys = w->iota + align256((size_t)n_edges * 4);
-    w->cub = w->keys + align256((size_t)n_edges * 4);
-    w->total = w->cub + align256(w->cub_bytes) + 256;
+static int layout(int64_t n_out, int64_t n_in, int64_t n_edges, void* base, GraphWs* w) {
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::InclusiveSum, (const int*)nullptr, (int*)nullptr, (int)n_out);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const int*)nullptr, (int*)nullptr, (const int*)nullptr,
+                  (int*)nullptr, (int)n_edges, 0, key_bits(n_in));
+    Planner p(base);
+    w->degs32 = p.take<int>(n_out);
+    w->iota = p.take<int>(n_edges);
+    w->keys = p.take<int>(n_edges);
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
 
@@ -107,12 +104,11 @@ extern "C" {
 
 int spg_graph_build_workspace(int64_t n_out, int64_t n_in, int64_t n_edges, int64_t* bytes) {
     if (!bytes || n_out < 0 || n_in < 0 || n_edges < 0) return SPG_E_BADARG;
-    if (n_out >= (1ll << 31) - 1 || n_in >= (1ll << 31) - 1 || n_edges >= (1ll << 31) - 1) return SPG_E_UNSUPPORTED;
+    if (too_big(n_out) || too_big(n_in) || too_big(n_edges)) return SPG_E_UNSUPPORTED;
     GraphWs w;
-    const int rc = plan(n_out, n_in, n_edges, &w);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)w.total;
-    return SPG_OK;
+    const int rc = layout(n_out, n_in, n_edges, nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_graph_build(const int64_t* idxn, const int64_t* degs, int64_t n_out, int64_t n_in, int64_t n_edges,
@@ -120,41 +116,29 @@ int spg_graph_build(const int64_t* idxn, const int64_t* degs, int64_t n_out, int
                     int32_t* src_perm, int32_t* status, void* workspace, int64_t workspace_bytes,
                     spg_stream_t stream) {
     if (n_out < 0 || n_in < 0 || n_edges < 0) return SPG_E_BADARG;
-    if (n_out >= (1ll << 31) - 1 || n_in >= (1ll << 31) - 1 || n_edges >= (1ll << 31) - 1) return SPG_E_UNSUPPORTED;
-    if (!tgt_rowptr || !src_rowptr || !status || !workspace) return SPG_E_BADARG;
+    if (too_big(n_out) || too_big(n_in) || too_big(n_edges)) return SPG_E_UNSUPPORTED;
+    if (!tgt_rowptr || !src_rowptr || !status) return SPG_E_BADARG;
     if ((n_edges > 0 && (!idxn || !idxn32 || !edge_tgt || !src_perm)) || (n_out > 0 && !degs)) return SPG_E_BADARG;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
     GraphWs w;
-    int rc = plan(n_out, n_in, n_edges, &w);
+    int rc = layout(n_out, n_in, n_edges, workspace, &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    int* degs32 = reinterpret_cast<int*>(ws + w.degs32);
-    int* iota = reinterpret_cast<int*>(ws + w.iota);
-    int* keys = reinterpret_cast<int*>(ws + w.keys);
-    void* cub_ws = ws + w.cub;
-    size_t cub_bytes = w.cub_bytes;
 
     cudaError_t e = cudaMemsetAsync(status, 0, sizeof(int), s);
     if (e != cudaSuccess) return (int)e;
     const int64_t n_max = (n_edges > n_out ? n_edges : n_out) > 0 ? (n_edges > n_out ? n_edges : n_out) : 1;
     SPG_LAUNCH(K_GRAPH_BUILD, s, graph_prepare_kernel, (unsigned)ceil_div64(n_max, GB_THREADS), GB_THREADS, 0,
-               idxn, degs, n_out, n_in, n_edges, idxn32, iota, degs32, tgt_rowptr, status);
-    if (n_out > 0) {
-        e = cub::DeviceScan::InclusiveSum(cub_ws, cub_bytes, (const int*)degs32, tgt_rowptr + 1, (int)n_out, s);
-        if (e != cudaSuccess) return (int)e;
-    }
+               idxn, degs, n_out, n_in, n_edges, idxn32, w.iota, w.degs32, tgt_rowptr, status);
+    if (n_out > 0)
+        SPG_CUB(w.cub, cub::DeviceScan::InclusiveSum, (const int*)w.degs32, tgt_rowptr + 1, (int)n_out, s);
     SPG_LAUNCH(K_GRAPH_BUILD, s, graph_edge_tgt_kernel, (unsigned)ceil_div64(n_edges > 0 ? n_edges : 1, GB_THREADS),
                GB_THREADS, 0, (const int*)tgt_rowptr, n_out, n_edges, edge_tgt, status);
-    if (n_edges > 0) {
-        cub_bytes = w.cub_bytes;
-        e = cub::DeviceRadixSort::SortPairs(cub_ws, cub_bytes, (const int*)idxn32, keys, (const int*)iota, src_perm,
-                                            (int)n_edges, 0, key_bits(n_in), s);
-        if (e != cudaSuccess) return (int)e;
-    }
+    if (n_edges > 0)
+        SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const int*)idxn32, w.keys, (const int*)w.iota, src_perm,
+                (int)n_edges, 0, key_bits(n_in), s);
     SPG_LAUNCH(K_GRAPH_BUILD, s, graph_src_rowptr_kernel, (unsigned)ceil_div64(n_in + 1, GB_THREADS), GB_THREADS, 0,
-               (const int*)keys, n_in, n_edges, src_rowptr);
+               (const int*)w.keys, n_in, n_edges, src_rowptr);
     return launch_status();
 }
 

@@ -23,7 +23,7 @@
 
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "workspace.cuh"
 
 namespace spg {
 
@@ -540,28 +540,50 @@ lp_perfect_kernel(const int64_t* __restrict__ comp_ptr, const int64_t* __restric
     }
 }
 
-static int sort_bytes_u64(int64_t n, size_t* bytes) {
-    size_t b = 0;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, b, (const unsigned long long*)nullptr,
-                                                    (unsigned long long*)nullptr, (const int*)nullptr, (int*)nullptr,
-                                                    (int)n, 0, 64);
-    if (e != cudaSuccess) return (int)e;
-    size_t b2 = 0;
-    e = cub::DeviceRadixSort::SortKeys(nullptr, b2, (const unsigned long long*)nullptr, (unsigned long long*)nullptr,
-                                       (int)n, 0, 64);
-    if (e != cudaSuccess) return (int)e;
-    size_t b3 = 0;
-    e = cub::DeviceRadixSort::SortPairs(nullptr, b3, (const int*)nullptr, (int*)nullptr, (const int*)nullptr,
-                                        (int*)nullptr, (int)n, 0, 32);
-    if (e != cudaSuccess) return (int)e;
-    size_t b4 = 0;
-    e = cub::DeviceScan::ExclusiveSum(nullptr, b4, (const int*)nullptr, (int*)nullptr, (int)n);
-    if (e != cudaSuccess) return (int)e;
-    *bytes = std::max(std::max(b, b2), std::max(b3, b4));
+// 2E incidence entries must fit in int32: a lower limit than too_big (workspace.cuh)
+static bool lp_too_big(int64_t n) { return n >= (1ll << 30); }
+
+// The scratch of spg_lp_incidence, spg_lp_xpart and spg_lp_seal; each call uses its own regions
+struct LpWs {
+    int *inc_keys, *inc_keys_sorted, *inc_vals;             // incidence [2E]
+    int *parent, *is_root, *root_rank;                      // xpart [V]
+    unsigned long long *pair_keys, *pair_keys_sorted;       // xpart [E]
+    int *pair_vals, *pair_vals_sorted;                      // xpart [E]
+    unsigned long long *comp_keys, *comp_keys_sorted;       // seal [V]
+    unsigned *size, *maxfreq;                               // seal [n_comp]
+    CubRegion cub;
+    size_t bytes;
+};
+
+static int layout(int64_t n_ver, int64_t n_edges, int64_t n_comp, void* base, LpWs* w) {
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const unsigned long long*)nullptr,
+                  (unsigned long long*)nullptr, (const int*)nullptr, (int*)nullptr, (int)n_edges, 0,
+                  bits_for((uint64_t)n_ver * (uint64_t)n_ver + 1));
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortKeys, (const unsigned long long*)nullptr,
+                  (unsigned long long*)nullptr, (int)n_ver, 0, 32 + bits_for((uint64_t)n_comp + 1));
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const int*)nullptr, (int*)nullptr,
+                  (const int*)nullptr, (int*)nullptr, (int)(2 * n_edges), 0, bits_for((uint64_t)n_ver + 1));
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::ExclusiveSum, (const int*)nullptr, (int*)nullptr, (int)n_ver);
+    Planner p(base);
+    w->inc_keys = p.take<int>(2 * n_edges);
+    w->inc_keys_sorted = p.take<int>(2 * n_edges);
+    w->inc_vals = p.take<int>(2 * n_edges);
+    w->parent = p.take<int>(n_ver);
+    w->is_root = p.take<int>(n_ver);
+    w->root_rank = p.take<int>(n_ver);
+    w->pair_keys = p.take<unsigned long long>(n_edges);
+    w->pair_keys_sorted = p.take<unsigned long long>(n_edges);
+    w->pair_vals = p.take<int>(n_edges);
+    w->pair_vals_sorted = p.take<int>(n_edges);
+    w->comp_keys = p.take<unsigned long long>(n_ver);
+    w->comp_keys_sorted = p.take<unsigned long long>(n_ver);
+    w->size = p.take<unsigned>(n_comp);
+    w->maxfreq = p.take<unsigned>(n_comp);
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
-
-static bool too_big(int64_t n) { return n >= (1ll << 30); }
 
 }  // namespace spg
 
@@ -569,34 +591,34 @@ using namespace spg;
 
 extern "C" {
 
-int spg_lp_sort_workspace(int64_t n, int64_t* bytes) {
-    if (!bytes || n < 0) return SPG_E_BADARG;
-    if (too_big(n)) return SPG_E_UNSUPPORTED;
-    size_t b = 0;
-    const int rc = sort_bytes_u64(n > 0 ? n : 1, &b);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)b + 256;
-    return SPG_OK;
+int spg_lp_workspace(int64_t n_ver, int64_t n_edges, int64_t n_comp, int64_t* bytes) {
+    if (!bytes || n_ver < 0 || n_edges < 0 || n_comp < 0) return SPG_E_BADARG;
+    if (lp_too_big(n_ver) || lp_too_big(2 * n_edges) || n_comp >= (1ll << 31)) return SPG_E_UNSUPPORTED;
+    LpWs w;
+    const int rc = layout(n_ver, n_edges, n_comp, nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_lp_incidence(const int64_t* src, const int64_t* tgt, int64_t n_ver, int64_t n_edges, int32_t* rowptr,
-                     int32_t* entry, int32_t* keys_tmp, int32_t* keys_sorted, int32_t* vals_tmp, void* workspace,
-                     int64_t workspace_bytes, spg_stream_t stream) {
+                     int32_t* entry, void* workspace, int64_t workspace_bytes, spg_stream_t stream) {
     if (n_ver < 0 || n_edges < 0 || !rowptr) return SPG_E_BADARG;
-    if (too_big(2 * n_edges) || too_big(n_ver)) return SPG_E_UNSUPPORTED;
+    if (lp_too_big(2 * n_edges) || lp_too_big(n_ver)) return SPG_E_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     const int64_t n = 2 * n_edges;
+    LpWs w;
+    int rc = layout(n_ver, n_edges, 0, workspace, &w);
+    if (rc != SPG_OK) return rc;
     if (n > 0) {
-        if (!src || !tgt || !entry || !keys_tmp || !keys_sorted || !vals_tmp || !workspace) return SPG_E_BADARG;
+        if (!src || !tgt || !entry) return SPG_E_BADARG;
+        rc = ws_check(workspace, workspace_bytes, w.bytes);
+        if (rc != SPG_OK) return rc;
         SPG_LAUNCH(K_LP_INCIDENCE, s, lp_incidence_keys_kernel, grid_of(n), LP_THREADS, 0, src, tgt, n_ver, n_edges,
-                   (int*)keys_tmp, (int*)vals_tmp);
-        size_t b = (size_t)workspace_bytes;
-        cudaError_t e = cub::DeviceRadixSort::SortPairs(workspace, b, (const int*)keys_tmp, (int*)keys_sorted,
-                                                        (const int*)vals_tmp, (int*)entry, (int)n, 0,
-                                                        bits_for((uint64_t)n_ver + 1), s);
-        if (e != cudaSuccess) return (int)e;
+                   w.inc_keys, w.inc_vals);
+        SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const int*)w.inc_keys, w.inc_keys_sorted,
+                (const int*)w.inc_vals, (int*)entry, (int)n, 0, bits_for((uint64_t)n_ver + 1), s);
     }
-    SPG_LAUNCH(K_LP_INCIDENCE, s, lp_rowptr_kernel, grid_of(n_ver + 1), LP_THREADS, 0, (const int*)keys_sorted,
+    SPG_LAUNCH(K_LP_INCIDENCE, s, lp_rowptr_kernel, grid_of(n_ver + 1), LP_THREADS, 0, (const int*)w.inc_keys_sorted,
                n_ver, n, (int*)rowptr);
     return launch_status();
 }
@@ -650,80 +672,76 @@ int spg_lp_loss_bwd(const float* diff, const float* weights, const uint8_t* is_t
 
 int spg_lp_xpart(const int64_t* src, const int64_t* tgt, const uint8_t* is_transition,
                  const int64_t* pred_in_component, int64_t n_ver, int64_t n_edges, double transition_factor,
-                 float* weights, int32_t* in_component_x, int32_t* comp_size, int32_t* n_comp, int32_t* parent,
-                 int32_t* is_root, int32_t* root_rank, uint64_t* keys_tmp, uint64_t* keys_sorted, int32_t* vals_tmp,
-                 int32_t* vals_sorted, void* workspace, int64_t workspace_bytes, spg_stream_t stream) {
+                 float* weights, int32_t* in_component_x, int32_t* comp_size, int32_t* n_comp, void* workspace,
+                 int64_t workspace_bytes, spg_stream_t stream) {
     if (n_ver < 0 || n_edges < 0 || !n_comp) return SPG_E_BADARG;
-    if (too_big(n_ver) || too_big(n_edges)) return SPG_E_UNSUPPORTED;
+    if (lp_too_big(n_ver) || lp_too_big(n_edges)) return SPG_E_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     cudaError_t e;
     if (n_ver == 0) {
         e = cudaMemsetAsync(n_comp, 0, sizeof(int32_t), s);
         if (e != cudaSuccess) return (int)e;
     }
-    if (n_ver > 0 && (!pred_in_component || !in_component_x || !comp_size || !parent || !is_root || !root_rank ||
-                      !workspace))
-        return SPG_E_BADARG;
-    if (n_edges > 0 && (!src || !tgt || !is_transition || !weights || !keys_tmp || !keys_sorted || !vals_tmp ||
-                        !vals_sorted || !workspace))
-        return SPG_E_BADARG;
+    if (n_ver > 0 && (!pred_in_component || !in_component_x || !comp_size)) return SPG_E_BADARG;
+    if (n_edges > 0 && (!src || !tgt || !is_transition || !weights)) return SPG_E_BADARG;
     const int64_t nmax = n_ver > n_edges ? n_ver : n_edges;
     if (nmax == 0) return SPG_OK;
+    LpWs w;
+    int rc = layout(n_ver, n_edges, 0, workspace, &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
+    if (rc != SPG_OK) return rc;
     SPG_LAUNCH(K_LP_CC, s, lp_cc_init_kernel, grid_of(nmax), LP_THREADS, 0, src, tgt, is_transition,
-               pred_in_component, n_ver, n_edges, (int*)parent, (int*)comp_size, weights);
+               pred_in_component, n_ver, n_edges, w.parent, (int*)comp_size, weights);
     if (n_ver == 0) return launch_status();
     if (n_edges > 0)
         SPG_LAUNCH(K_LP_CC, s, lp_cc_hook_kernel, grid_of(n_edges), LP_THREADS, 0, src, tgt, is_transition,
-                   pred_in_component, n_ver, n_edges, (int*)parent);
-    SPG_LAUNCH(K_LP_CC, s, lp_cc_flatten_kernel, grid_of(n_ver), LP_THREADS, 0, (int*)parent, n_ver, (int*)is_root);
-    size_t b = (size_t)workspace_bytes;
-    e = cub::DeviceScan::ExclusiveSum(workspace, b, (const int*)is_root, (int*)root_rank, (int)n_ver, s);
-    if (e != cudaSuccess) return (int)e;
-    SPG_LAUNCH(K_LP_CC, s, lp_cc_label_kernel, grid_of(n_ver), LP_THREADS, 0, (const int*)parent,
-               (const int*)root_rank, (const int*)is_root, n_ver, (int*)in_component_x, (int*)comp_size, (int*)n_comp);
+                   pred_in_component, n_ver, n_edges, w.parent);
+    SPG_LAUNCH(K_LP_CC, s, lp_cc_flatten_kernel, grid_of(n_ver), LP_THREADS, 0, w.parent, n_ver, w.is_root);
+    SPG_CUB(w.cub, cub::DeviceScan::ExclusiveSum, (const int*)w.is_root, w.root_rank, (int)n_ver, s);
+    SPG_LAUNCH(K_LP_CC, s, lp_cc_label_kernel, grid_of(n_ver), LP_THREADS, 0, (const int*)w.parent,
+               (const int*)w.root_rank, (const int*)w.is_root, n_ver, (int*)in_component_x, (int*)comp_size,
+               (int*)n_comp);
     if (n_edges == 0) return launch_status();
     SPG_LAUNCH(K_LP_XPART, s, lp_xpart_keys_kernel, grid_of(n_edges), LP_THREADS, 0, src, tgt, is_transition,
-               (const int*)in_component_x, n_ver, n_edges, (unsigned long long*)keys_tmp, (int*)vals_tmp);
-    b = (size_t)workspace_bytes;
-    e = cub::DeviceRadixSort::SortPairs(workspace, b, (const unsigned long long*)keys_tmp,
-                                        (unsigned long long*)keys_sorted, (const int*)vals_tmp, (int*)vals_sorted,
-                                        (int)n_edges, 0, bits_for((uint64_t)n_ver * (uint64_t)n_ver + 1), s);
-    if (e != cudaSuccess) return (int)e;
+               (const int*)in_component_x, n_ver, n_edges, w.pair_keys, w.pair_vals);
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const unsigned long long*)w.pair_keys, w.pair_keys_sorted,
+            (const int*)w.pair_vals, w.pair_vals_sorted, (int)n_edges, 0,
+            bits_for((uint64_t)n_ver * (uint64_t)n_ver + 1), s);
     SPG_LAUNCH(K_LP_XPART, s, lp_xpart_weights_kernel, grid_of(n_edges), LP_THREADS, 0,
-               (const unsigned long long*)keys_sorted, (const int*)vals_sorted, n_ver, n_edges,
+               (const unsigned long long*)w.pair_keys_sorted, (const int*)w.pair_vals_sorted, n_ver, n_edges,
                (const int*)comp_size, transition_factor, weights);
     return launch_status();
 }
 
 int spg_lp_seal(const int64_t* src, const int64_t* tgt, const uint8_t* is_transition, const int64_t* pred_in_component,
                 const int64_t* objects, int64_t n_ver, int64_t n_edges, int64_t n_comp, double transition_factor,
-                float* weights, int32_t* w_per_component, int32_t* size_tmp, int32_t* maxfreq_tmp, uint64_t* keys_tmp,
-                uint64_t* keys_sorted, void* workspace, int64_t workspace_bytes, spg_stream_t stream) {
+                float* weights, int32_t* w_per_component, void* workspace, int64_t workspace_bytes,
+                spg_stream_t stream) {
     if (n_ver < 0 || n_edges < 0 || n_comp < 0) return SPG_E_BADARG;
-    if (too_big(n_ver) || too_big(n_edges) || n_comp >= (1ll << 31)) return SPG_E_UNSUPPORTED;
+    if (lp_too_big(n_ver) || lp_too_big(n_edges) || n_comp >= (1ll << 31)) return SPG_E_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     const int64_t nmax = std::max(n_ver, n_comp);
+    LpWs w;
+    int rc = layout(n_ver, n_edges, n_comp, workspace, &w);
+    if (rc != SPG_OK) return rc;
     if (nmax > 0) {
-        if (!size_tmp || !maxfreq_tmp || (n_ver > 0 && (!pred_in_component || !objects || !keys_tmp || !keys_sorted ||
-                                                       !workspace)))
-            return SPG_E_BADARG;
+        if (n_ver > 0 && (!pred_in_component || !objects)) return SPG_E_BADARG;
+        rc = ws_check(workspace, workspace_bytes, w.bytes);
+        if (rc != SPG_OK) return rc;
         SPG_LAUNCH(K_LP_SEAL, s, lp_seal_keys_kernel, grid_of(nmax), LP_THREADS, 0, pred_in_component, objects, n_ver,
-                   n_comp, (unsigned long long*)keys_tmp, (unsigned*)size_tmp, (unsigned*)maxfreq_tmp);
+                   n_comp, w.comp_keys, w.size, w.maxfreq);
     }
     if (n_ver > 0) {
-        size_t b = (size_t)workspace_bytes;
-        cudaError_t e = cub::DeviceRadixSort::SortKeys(workspace, b, (const unsigned long long*)keys_tmp,
-                                                       (unsigned long long*)keys_sorted, (int)n_ver, 0,
-                                                       32 + bits_for((uint64_t)n_comp + 1), s);
-        if (e != cudaSuccess) return (int)e;
+        SPG_CUB(w.cub, cub::DeviceRadixSort::SortKeys, (const unsigned long long*)w.comp_keys, w.comp_keys_sorted,
+                (int)n_ver, 0, 32 + bits_for((uint64_t)n_comp + 1), s);
         SPG_LAUNCH(K_LP_SEAL, s, lp_seal_runs_kernel, grid_of(n_ver), LP_THREADS, 0,
-                   (const unsigned long long*)keys_sorted, n_ver, n_comp, (unsigned*)size_tmp, (unsigned*)maxfreq_tmp);
+                   (const unsigned long long*)w.comp_keys_sorted, n_ver, n_comp, w.size, w.maxfreq);
     }
     const int64_t n2 = std::max(n_edges, w_per_component ? n_comp : 0);
     if (n2 == 0) return launch_status();
     if (n_edges > 0 && (!src || !tgt || !is_transition || !weights)) return SPG_E_BADARG;
     SPG_LAUNCH(K_LP_SEAL, s, lp_seal_weights_kernel, grid_of(n2), LP_THREADS, 0, src, tgt, is_transition,
-               pred_in_component, n_ver, n_edges, n_comp, (const unsigned*)size_tmp, (const unsigned*)maxfreq_tmp,
+               pred_in_component, n_ver, n_edges, n_comp, (const unsigned*)w.size, (const unsigned*)w.maxfreq,
                transition_factor, weights, w_per_component);
     return launch_status();
 }

@@ -16,7 +16,7 @@
 // the reference; the rotation is BLAS's float32 matmul on the host, whose last bit is not promised.
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "workspace.cuh"
 #include "philox.cuh"
 
 namespace spg {
@@ -279,28 +279,25 @@ __global__ void __launch_bounds__(kLclWarps * 32) lp_local_clouds_kernel(const L
         a.labels_out[i * a.n_label_cols + c] = (int64_t)__ldg(a.labels + v * a.n_label_cols + c);
 }
 
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct SubgraphWs {
-    size_t vflag, eflag, cub, total, cub_bytes;
+    int *vflag, *eflag;
+    CubRegion cub;
+    size_t bytes;
 };
 
-static int plan(int64_t n_ver, int64_t n_edges, SubgraphWs* w) {
-    size_t a = 0, b = 0;
-    cudaError_t e = cub::DeviceScan::InclusiveSum(nullptr, a, (const int*)nullptr, (int*)nullptr,
-                                                  (int)(n_ver > 0 ? n_ver : 1));
-    if (e != cudaSuccess) return (int)e;
-    e = cub::DeviceScan::InclusiveSum(nullptr, b, (const int*)nullptr, (int*)nullptr, (int)(n_edges > 0 ? n_edges : 1));
-    if (e != cudaSuccess) return (int)e;
-    w->cub_bytes = a > b ? a : b;
-    w->vflag = 0;
-    w->eflag = align256((size_t)n_ver * 4);
-    w->cub = w->eflag + align256((size_t)n_edges * 4);
-    w->total = w->cub + align256(w->cub_bytes) + 256;
+static int layout(int64_t n_ver, int64_t n_edges, void* base, SubgraphWs* w) {
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::InclusiveSum, (const int*)nullptr, (int*)nullptr,
+                  (int)(n_ver > 0 ? n_ver : 1));
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::InclusiveSum, (const int*)nullptr, (int*)nullptr,
+                  (int)(n_edges > 0 ? n_edges : 1));
+    Planner p(base);
+    w->vflag = p.take<int>(n_ver);
+    w->eflag = p.take<int>(n_edges);
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
-
-static bool too_big(int64_t n) { return n >= (1ll << 31) - 1; }
 
 }  // namespace spg
 
@@ -343,10 +340,9 @@ int spg_lp_subgraph_workspace(int64_t n_ver, int64_t n_edges, int64_t* bytes) {
     if (!bytes || n_ver < 0 || n_edges < 0) return SPG_E_BADARG;
     if (too_big(n_ver) || too_big(n_edges)) return SPG_E_UNSUPPORTED;
     SubgraphWs w;
-    const int rc = plan(n_ver, n_edges, &w);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)w.total;
-    return SPG_OK;
+    const int rc = layout(n_ver, n_edges, nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_lp_subgraph_select(const uint8_t* mask, const int32_t* objects, int64_t n_ver, const int32_t* src,
@@ -360,33 +356,23 @@ int spg_lp_subgraph_select(const uint8_t* mask, const int32_t* objects, int64_t 
     if (e != cudaSuccess) return (int)e;
     if (n_ver > 0 && !objects) return SPG_E_BADARG;
     if (mask) {
-        if (!new_index || !edge_pos || !workspace || (n_ver > 0 && !selected) || (n_edges > 0 && (!src || !tgt)))
+        if (!new_index || !edge_pos || (n_ver > 0 && !selected) || (n_edges > 0 && (!src || !tgt)))
             return SPG_E_BADARG;
-        if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
         SubgraphWs w;
-        int rc = plan(n_ver, n_edges, &w);
+        int rc = layout(n_ver, n_edges, workspace, &w);
+        if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
         if (rc != SPG_OK) return rc;
-        if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
-        uint8_t* ws = static_cast<uint8_t*>(workspace);
-        int* vflag = reinterpret_cast<int*>(ws + w.vflag);
-        int* eflag = reinterpret_cast<int*>(ws + w.eflag);
         e = cudaMemsetAsync(new_index, 0, sizeof(int), s);
         if (e == cudaSuccess) e = cudaMemsetAsync(edge_pos, 0, sizeof(int), s);
         if (e != cudaSuccess) return (int)e;
         const int64_t nm = n_ver > n_edges ? n_ver : n_edges;
         if (nm > 0)
             SPG_LAUNCH(K_LP_SUBGRAPH, s, lp_subgraph_flags_kernel, (unsigned)ceil_div64(nm, LPL_THREADS), LPL_THREADS,
-                       0, mask, n_ver, src, tgt, n_edges, vflag, eflag);
-        size_t cb = w.cub_bytes;
-        if (n_ver > 0) {
-            e = cub::DeviceScan::InclusiveSum(ws + w.cub, cb, (const int*)vflag, new_index + 1, (int)n_ver, s);
-            if (e != cudaSuccess) return (int)e;
-        }
-        cb = w.cub_bytes;
-        if (n_edges > 0) {
-            e = cub::DeviceScan::InclusiveSum(ws + w.cub, cb, (const int*)eflag, edge_pos + 1, (int)n_edges, s);
-            if (e != cudaSuccess) return (int)e;
-        }
+                       0, mask, n_ver, src, tgt, n_edges, w.vflag, w.eflag);
+        if (n_ver > 0)
+            SPG_CUB(w.cub, cub::DeviceScan::InclusiveSum, (const int*)w.vflag, new_index + 1, (int)n_ver, s);
+        if (n_edges > 0)
+            SPG_CUB(w.cub, cub::DeviceScan::InclusiveSum, (const int*)w.eflag, edge_pos + 1, (int)n_edges, s);
     }
     if (n_ver > 0)
         SPG_LAUNCH(K_LP_SUBGRAPH, s, lp_subgraph_vertices_kernel, (unsigned)ceil_div64(n_ver, LPL_THREADS),

@@ -18,21 +18,11 @@
 // No float atomics anywhere: two runs give identical bits.
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "workspace.cuh"
 
 namespace spg {
 
 constexpr int PR_THREADS = 256;
-
-// order-preserving map float -> uint32 (-0 below +0, as the reference's `<` does not order them: either may be the
-// minimum, and both give the same bins)
-__device__ __forceinline__ unsigned pr_fkey(float f) {
-    const unsigned u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float pr_funkey(unsigned k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
 
 // the reference's bin: (uint32) floor((x - x_min) / voxel), every step in fp32 (ply_c.cpp:329-331)
 __device__ __forceinline__ float pr_binf(float x, float lo, float voxel) {
@@ -53,9 +43,9 @@ struct PruneGeom {
 __device__ __forceinline__ void pr_key(const PruneGeom& g, int64_t i, uint64_t& lo, uint64_t& hi) {
     const int64_t c = i / g.chunk_rows;
     const unsigned* b = g.bounds + 6 * c;
-    const unsigned bx = (unsigned)pr_binf(__ldg(g.xyz + 3 * i), pr_funkey(~__ldg(b)), g.voxel);
-    const unsigned by = (unsigned)pr_binf(__ldg(g.xyz + 3 * i + 1), pr_funkey(~__ldg(b + 1)), g.voxel);
-    const unsigned bz = (unsigned)pr_binf(__ldg(g.xyz + 3 * i + 2), pr_funkey(~__ldg(b + 2)), g.voxel);
+    const unsigned bx = (unsigned)pr_binf(__ldg(g.xyz + 3 * i), float_unkey(~__ldg(b)), g.voxel);
+    const unsigned by = (unsigned)pr_binf(__ldg(g.xyz + 3 * i + 1), float_unkey(~__ldg(b + 1)), g.voxel);
+    const unsigned bz = (unsigned)pr_binf(__ldg(g.xyz + 3 * i + 2), float_unkey(~__ldg(b + 2)), g.voxel);
     unsigned __int128 k = (unsigned __int128)c;
     k = (k << g.bits_x) | bx;
     k = (k << g.bits_y) | by;
@@ -85,7 +75,8 @@ __global__ void __launch_bounds__(PR_THREADS) prune_bounds_kernel(const float* _
                 bad |= 1u;
                 continue;
             }
-            const unsigned key = pr_fkey(v);
+            // -0 keys below +0; the reference's `<` does not order them, so either may be the minimum: both give the same bins
+            const unsigned key = float_key(v);
             lo[k] = min(lo[k], key);
             hi[k] = max(hi[k], key);
         }
@@ -134,7 +125,7 @@ __global__ void __launch_bounds__(PR_THREADS) prune_bins_kernel(const unsigned* 
             const unsigned klo = ~__ldg(bounds + 6 * c + k), khi = __ldg(bounds + 6 * c + 3 + k);
             if (klo == ~0u) continue;  // no finite coordinate (reported by status 1)
             // the bins are monotone in x, so the chunk's largest bin is the bin of its maximum
-            const float b = pr_binf(pr_funkey(khi), pr_funkey(klo), voxel);
+            const float b = pr_binf(float_unkey(khi), float_unkey(klo), voxel);
             if (!(b < 4294967296.f)) {
                 atomicOr(&s_bad, 2u);
                 continue;
@@ -316,43 +307,41 @@ __global__ void __launch_bounds__(PR_THREADS) prune_hist_kernel(const int32_t* _
 }
 
 // ------------------------------------------------------------------------------------------------ plan
-static size_t pr_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct PruneWs {
-    size_t bounds, status, keys_in, keys, idx_in, idx, head, first, run_of, row_of, run_start, run_row, xyz_s, rgb_s,
-        cub, total, cub_bytes;
+    unsigned *bounds, *status;
+    uint64_t *keys_in, *keys;
+    int32_t *idx_in, *idx, *head, *first, *run_of, *row_of, *run_start, *run_row;
+    float* xyz_s;
+    uint32_t* rgb_s;
+    CubRegion cub;
+    size_t bytes;
 };
 
-static int plan_prune(int64_t n, int64_t n_chunks, PruneWs* w) {
+static int layout(int64_t n, int64_t n_chunks, void* base, PruneWs* w) {
     const int m = (int)(n > 0 ? n : 1);
-    size_t b[3] = {0, 0, 0};
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, b[0], (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                                    (const int32_t*)nullptr, (int32_t*)nullptr, m);
-    if (e == cudaSuccess)
-        e = cub::DeviceScan::ExclusiveSum(nullptr, b[1], (const int32_t*)nullptr, (int32_t*)nullptr, m);
-    if (e == cudaSuccess)
-        e = cub::DeviceScan::InclusiveSum(nullptr, b[2], (const int32_t*)nullptr, (int32_t*)nullptr, m);
-    if (e != cudaSuccess) return (int)e;
-    w->cub_bytes = 0;
-    for (size_t x : b) w->cub_bytes = x > w->cub_bytes ? x : w->cub_bytes;
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (const int32_t*)nullptr, (int32_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::ExclusiveSum, (const int32_t*)nullptr, (int32_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::InclusiveSum, (const int32_t*)nullptr, (int32_t*)nullptr, m);
     const size_t N = (size_t)m, C = (size_t)(n_chunks > 0 ? n_chunks : 1);
-    size_t o = 0;
-    w->bounds = o;     o += pr_align(C * 6 * 4);
-    w->status = o;     o += 256;
-    w->keys_in = o;    o += pr_align(N * 8);
-    w->keys = o;       o += pr_align(N * 8);
-    w->idx_in = o;     o += pr_align(N * 4);
-    w->idx = o;        o += pr_align(N * 4);
-    w->head = o;       o += pr_align(N * 4);
-    w->first = o;      o += pr_align(N * 4);
-    w->run_of = o;     o += pr_align(N * 4);
-    w->row_of = o;     o += pr_align(N * 4);
-    w->run_start = o;  o += pr_align((N + 1) * 4);
-    w->run_row = o;    o += pr_align(N * 4);
-    w->xyz_s = o;      o += pr_align(N * 12);
-    w->rgb_s = o;      o += pr_align(N * 4);
-    w->cub = o;        o += pr_align(w->cub_bytes);
-    w->total = o;
+    Planner p(base);
+    w->bounds = p.take<unsigned>(C * 6);
+    w->status = p.take<unsigned>(1);
+    w->keys_in = p.take<uint64_t>(N);
+    w->keys = p.take<uint64_t>(N);
+    w->idx_in = p.take<int32_t>(N);
+    w->idx = p.take<int32_t>(N);
+    w->head = p.take<int32_t>(N);
+    w->first = p.take<int32_t>(N);
+    w->run_of = p.take<int32_t>(N);
+    w->row_of = p.take<int32_t>(N);
+    w->run_start = p.take<int32_t>(N + 1);
+    w->run_row = p.take<int32_t>(N);
+    w->xyz_s = p.take<float>(3 * N);
+    w->rgb_s = p.take<uint32_t>(N);
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
 
@@ -367,13 +356,11 @@ static int64_t pr_chunks(int64_t n, int64_t chunk_rows) { return (n + chunk_rows
 // the chunk rows and the workspace of one call
 static int pr_setup(int64_t n, int64_t chunk_rows, void* workspace, int64_t workspace_bytes, PruneWs* w,
                     int64_t* rows) {
-    if (n <= 0 || chunk_rows < 0 || !workspace) return SPG_E_BADARG;
-    if (n >= (1ll << 31) - 1) return SPG_E_UNSUPPORTED;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
+    if (n <= 0 || chunk_rows < 0) return SPG_E_BADARG;
+    if (too_big(n)) return SPG_E_UNSUPPORTED;
     *rows = chunk_rows == 0 || chunk_rows > n ? n : chunk_rows;
-    const int rc = plan_prune(n, pr_chunks(n, *rows), w);
-    if (rc != SPG_OK) return rc;
-    return workspace_bytes < (int64_t)w->total ? SPG_E_BADARG : SPG_OK;
+    const int rc = layout(n, pr_chunks(n, *rows), workspace, w);
+    return rc == SPG_OK ? ws_check(workspace, workspace_bytes, w->bytes) : rc;
 }
 
 }  // namespace spg
@@ -384,13 +371,12 @@ extern "C" {
 
 int spg_prune_workspace(int64_t n, int64_t chunk_rows, int64_t* bytes) {
     if (!bytes || n <= 0 || chunk_rows < 0) return SPG_E_BADARG;
-    if (n >= (1ll << 31) - 1) return SPG_E_UNSUPPORTED;
+    if (too_big(n)) return SPG_E_UNSUPPORTED;
     const int64_t rows = chunk_rows == 0 || chunk_rows > n ? n : chunk_rows;
     PruneWs w;
-    const int rc = plan_prune(n, pr_chunks(n, rows), &w);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)w.total;
-    return SPG_OK;
+    const int rc = layout(n, pr_chunks(n, rows), nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_prune_bounds(const float* xyz, int64_t n, int64_t chunk_rows, float voxel_size, const int64_t* labels,
@@ -406,11 +392,8 @@ int spg_prune_bounds(const float* xyz, int64_t n, int64_t chunk_rows, float voxe
     const int64_t C = pr_chunks(n, rows);
     if (C > 65535) return SPG_E_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    unsigned* bounds = reinterpret_cast<unsigned*>(ws + w.bounds);
-    unsigned* status = reinterpret_cast<unsigned*>(ws + w.status);
-    cudaError_t e = cudaMemsetAsync(bounds, 0, (size_t)C * 6 * 4, s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(status, 0, 4, s);
+    cudaError_t e = cudaMemsetAsync(w.bounds, 0, (size_t)C * 6 * 4, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(w.status, 0, 4, s);
     if (e != cudaSuccess) return (int)e;
     const int64_t per = ceil_div64(rows, PR_THREADS);
     const int64_t cap = (4 * kNumSMs + C - 1) / C;
@@ -418,9 +401,10 @@ int spg_prune_bounds(const float* xyz, int64_t n, int64_t chunk_rows, float voxe
     const bool with_labels = n_labels > 0;
     SPG_LAUNCH(K_PRUNE_BOUNDS, s, prune_bounds_kernel, grid, PR_THREADS, 0, xyz, n, rows,
                with_labels ? labels : (const int64_t*)nullptr,
-               with_labels && n_objects > 0 ? objects : (const int64_t*)nullptr, n_labels, n_objects, bounds, status);
-    SPG_LAUNCH(K_PRUNE_BOUNDS, s, prune_bins_kernel, 1, PR_THREADS, 0, (const unsigned*)bounds, C, voxel_size,
-               (const unsigned*)status, (unsigned long long*)words);
+               with_labels && n_objects > 0 ? objects : (const int64_t*)nullptr, n_labels, n_objects, w.bounds,
+               w.status);
+    SPG_LAUNCH(K_PRUNE_BOUNDS, s, prune_bins_kernel, 1, PR_THREADS, 0, (const unsigned*)w.bounds, C, voxel_size,
+               (const unsigned*)w.status, (unsigned long long*)words);
     return launch_status();
 }
 
@@ -435,59 +419,42 @@ int spg_prune_voxels(const float* xyz, int64_t n, int64_t chunk_rows, float voxe
     int rc = pr_setup(n, chunk_rows, workspace, workspace_bytes, &w, &rows);
     if (rc != SPG_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    uint64_t* keys_in = reinterpret_cast<uint64_t*>(ws + w.keys_in);
-    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + w.keys);
-    int32_t* idx_in = reinterpret_cast<int32_t*>(ws + w.idx_in);
-    int32_t* idx = reinterpret_cast<int32_t*>(ws + w.idx);
-    int32_t* head = reinterpret_cast<int32_t*>(ws + w.head);
-    int32_t* first = reinterpret_cast<int32_t*>(ws + w.first);
-    int32_t* run_of = reinterpret_cast<int32_t*>(ws + w.run_of);
-    int32_t* row_of = reinterpret_cast<int32_t*>(ws + w.row_of);
     PruneGeom g;
     g.xyz = xyz;
     g.n = n;
     g.chunk_rows = rows;
     g.voxel = voxel_size;
-    g.bounds = reinterpret_cast<const unsigned*>(ws + w.bounds);
+    g.bounds = w.bounds;
     g.bits_x = pr_bits(max_bin_x);
     g.bits_y = pr_bits(max_bin_y);
     g.bits_z = pr_bits(max_bin_z);
     g.bits_total = pr_bits(pr_chunks(n, rows) - 1) + g.bits_x + g.bits_y + g.bits_z;
     const unsigned blocks = (unsigned)ceil_div64(n, PR_THREADS);
     const int N = (int)n;
-    SPG_LAUNCH(K_PRUNE_KEYS, s, prune_keys_kernel<0>, blocks, PR_THREADS, 0, g, (const int32_t*)nullptr, keys_in,
-               idx_in);
-    size_t cb = w.cub_bytes;
+    SPG_LAUNCH(K_PRUNE_KEYS, s, prune_keys_kernel<0>, blocks, PR_THREADS, 0, g, (const int32_t*)nullptr, w.keys_in,
+               w.idx_in);
     const int lo_bits = g.bits_total < 64 ? (g.bits_total > 0 ? g.bits_total : 1) : 64;
-    cudaError_t e = cub::DeviceRadixSort::SortPairs(ws + w.cub, cb, (const uint64_t*)keys_in, keys,
-                                                    (const int32_t*)idx_in, idx, N, 0, lo_bits, s);
-    if (e != cudaSuccess) return (int)e;
-    const int32_t* order = idx;
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const uint64_t*)w.keys_in, w.keys, (const int32_t*)w.idx_in,
+            w.idx, N, 0, lo_bits, s);
+    const int32_t* order = w.idx;
     if (g.bits_total > 64) {  // LSD: the high bits last, stable, carrying the order of the first sort
-        SPG_LAUNCH(K_PRUNE_KEYS, s, prune_keys_kernel<1>, blocks, PR_THREADS, 0, g, (const int32_t*)idx, keys_in,
+        SPG_LAUNCH(K_PRUNE_KEYS, s, prune_keys_kernel<1>, blocks, PR_THREADS, 0, g, (const int32_t*)w.idx, w.keys_in,
                    (int32_t*)nullptr);
-        cb = w.cub_bytes;
-        e = cub::DeviceRadixSort::SortPairs(ws + w.cub, cb, (const uint64_t*)keys_in, keys, (const int32_t*)idx,
-                                            idx_in, N, 0, g.bits_total - 64, s);
-        if (e != cudaSuccess) return (int)e;
-        order = idx_in;
+        SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const uint64_t*)w.keys_in, w.keys, (const int32_t*)w.idx,
+                w.idx_in, N, 0, g.bits_total - 64, s);
+        order = w.idx_in;
     }
-    SPG_LAUNCH(K_PRUNE_ROWS, s, prune_heads_kernel, blocks, PR_THREADS, 0, g, order, head, first);
-    cb = w.cub_bytes;
-    e = cub::DeviceScan::ExclusiveSum(ws + w.cub, cb, (const int32_t*)first, row_of, N, s);
-    if (e != cudaSuccess) return (int)e;
-    cb = w.cub_bytes;
-    e = cub::DeviceScan::InclusiveSum(ws + w.cub, cb, (const int32_t*)head, run_of, N, s);
-    if (e != cudaSuccess) return (int)e;
+    SPG_LAUNCH(K_PRUNE_ROWS, s, prune_heads_kernel, blocks, PR_THREADS, 0, g, order, w.head, w.first);
+    SPG_CUB(w.cub, cub::DeviceScan::ExclusiveSum, (const int32_t*)w.first, w.row_of, N, s);
+    SPG_CUB(w.cub, cub::DeviceScan::InclusiveSum, (const int32_t*)w.head, w.run_of, N, s);
     // the final order goes to `idx` whichever sort produced it, for the reduce
-    if (order != idx) {
-        e = cudaMemcpyAsync(idx, order, (size_t)n * 4, cudaMemcpyDeviceToDevice, s);
+    if (order != w.idx) {
+        const cudaError_t e = cudaMemcpyAsync(w.idx, order, (size_t)n * 4, cudaMemcpyDeviceToDevice, s);
         if (e != cudaSuccess) return (int)e;
     }
-    SPG_LAUNCH(K_PRUNE_ROWS, s, prune_runs_kernel, blocks, PR_THREADS, 0, (const int32_t*)idx, (const int32_t*)head,
-               (const int32_t*)run_of, (const int32_t*)row_of, n, reinterpret_cast<int32_t*>(ws + w.run_start),
-               reinterpret_cast<int32_t*>(ws + w.run_row), n_voxels);
+    SPG_LAUNCH(K_PRUNE_ROWS, s, prune_runs_kernel, blocks, PR_THREADS, 0, (const int32_t*)w.idx,
+               (const int32_t*)w.head, (const int32_t*)w.run_of, (const int32_t*)w.row_of, n, w.run_start, w.run_row,
+               n_voxels);
     return launch_status();
 }
 
@@ -503,23 +470,16 @@ int spg_prune_reduce(const float* xyz, const uint8_t* rgb, const int64_t* labels
     const int rc = pr_setup(n, chunk_rows, const_cast<void*>(workspace), workspace_bytes, &w, &rows);
     if (rc != SPG_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(const_cast<void*>(workspace));
-    const int32_t* idx = reinterpret_cast<const int32_t*>(ws + w.idx);
-    const int32_t* run_of = reinterpret_cast<const int32_t*>(ws + w.run_of);
-    const int32_t* run_start = reinterpret_cast<const int32_t*>(ws + w.run_start);
-    const int32_t* run_row = reinterpret_cast<const int32_t*>(ws + w.run_row);
-    float* xyz_s = reinterpret_cast<float*>(ws + w.xyz_s);
-    uint32_t* rgb_s = reinterpret_cast<uint32_t*>(ws + w.rgb_s);
     cudaError_t e = cudaMemsetAsync(labels_out, 0, (size_t)n_voxels * (n_labels + 1) * 8, s);
     if (e == cudaSuccess) e = cudaMemsetAsync(objects_out, 0, (size_t)n_voxels * (n_objects + 1) * 8, s);
     if (e != cudaSuccess) return (int)e;
     const unsigned blocks = (unsigned)ceil_div64(n, PR_THREADS);
-    SPG_LAUNCH(K_PRUNE_REDUCE, s, prune_gather_kernel, blocks, PR_THREADS, 0, xyz, rgb, idx, n, xyz_s, rgb_s);
+    SPG_LAUNCH(K_PRUNE_REDUCE, s, prune_gather_kernel, blocks, PR_THREADS, 0, xyz, rgb, w.idx, n, w.xyz_s, w.rgb_s);
     SPG_LAUNCH(K_PRUNE_REDUCE, s, prune_reduce_kernel, (unsigned)ceil_div64(n_voxels, PR_THREADS), PR_THREADS, 0,
-               (const float*)xyz_s, (const uint32_t*)rgb_s, run_start, run_row, n_voxels, xyz_out, rgb_out);
+               (const float*)w.xyz_s, (const uint32_t*)w.rgb_s, w.run_start, w.run_row, n_voxels, xyz_out, rgb_out);
     // ply_c.cpp:343-354: the labels counted when n_labels > 0, the objects only with them
     if (n_labels > 0)
-        SPG_LAUNCH(K_PRUNE_REDUCE, s, prune_hist_kernel, blocks, PR_THREADS, 0, idx, run_of, run_row, n, labels,
+        SPG_LAUNCH(K_PRUNE_REDUCE, s, prune_hist_kernel, blocks, PR_THREADS, 0, w.idx, w.run_of, w.run_row, n, labels,
                    n_labels, n_objects > 0 ? objects : (const int64_t*)nullptr, n_objects, labels_out, objects_out);
     return launch_status();
 }

@@ -23,7 +23,7 @@
 // No float atomics anywhere: two runs give identical bits.
 #include <cub/cub.cuh>
 
-#include "common.cuh"
+#include "workspace.cuh"
 #include "eig3.cuh"
 
 namespace spg {
@@ -31,12 +31,6 @@ namespace spg {
 constexpr int SPG_THREADS = 256;
 constexpr int SP_WARPS = 8;  // components per block of sp_points
 constexpr uint64_t kNoKey = ~0ull;
-
-// order-preserving map float -> uint32, -0 mapped to +0
-__device__ __forceinline__ uint64_t sp_fkey(float f) {
-    const unsigned u = __float_as_uint(__fadd_rn(f, 0.f));
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 
 // ------------------------------------------------------------------------------------------------ scan
 // words[0] = max id + 1 (preset to 0), words[1] = status (preset to 0)
@@ -72,7 +66,9 @@ __global__ void __launch_bounds__(SPG_THREADS) sp_keys_lo_kernel(const float* __
     SPG_PDL_ENTRY();
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    keys[i] = (sp_fkey(__ldg(xyz + 3 * i + 1)) << 32) | sp_fkey(__ldg(xyz + 3 * i + 2));
+    // + 0.f maps -0 to +0
+    keys[i] = ((uint64_t)float_key(__fadd_rn(__ldg(xyz + 3 * i + 1), 0.f)) << 32) |
+              float_key(__fadd_rn(__ldg(xyz + 3 * i + 2), 0.f));
     idx[i] = (int32_t)i;
 }
 
@@ -84,7 +80,7 @@ __global__ void __launch_bounds__(SPG_THREADS) sp_keys_hi_kernel(const float* __
     const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= n) return;
     const int64_t i = __ldg(idx + p);
-    keys[p] = ((uint64_t)__ldg(comp + i) << 32) | sp_fkey(__ldg(xyz + 3 * i));
+    keys[p] = ((uint64_t)__ldg(comp + i) << 32) | float_key(__fadd_rn(__ldg(xyz + 3 * i), 0.f));
 }
 
 // start[c] = first sorted position of component c; an empty component gets the empty range [p, p)
@@ -429,73 +425,71 @@ __global__ void __launch_bounds__(SPG_THREADS) sp_edges_kernel(const EdgesArgs a
 }
 
 // ------------------------------------------------------------------------------------------------ plans
-static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 struct PointsWs {
-    size_t keys_in, keys, idx_in, idx, start, cub, total, cub_bytes;
+    uint64_t *keys_in, *keys;
+    int32_t *idx_in, *idx, *start;
+    CubRegion cub;
+    size_t bytes;
 };
 
-static int plan_points(int64_t n, PointsWs* w) {
+static int layout(int64_t n, void* base, PointsWs* w) {
     const int m = (int)(n > 0 ? n : 1);
-    size_t a = 0;
-    const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, a, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                                          (const int32_t*)nullptr, (int32_t*)nullptr, m);
-    if (e != cudaSuccess) return (int)e;
-    w->cub_bytes = a;
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (const int32_t*)nullptr, (int32_t*)nullptr, m);
     const size_t N = (size_t)m;
-    size_t o = 0;
-    w->keys_in = o;  o += align256(N * 8);
-    w->keys = o;     o += align256(N * 8);
-    w->idx_in = o;   o += align256(N * 4);
-    w->idx = o;      o += align256(N * 4);
-    w->start = o;    o += align256((N + 1) * 4);  // n_com <= n for a partition with no empty component
-    w->cub = o;      o += align256(w->cub_bytes);
-    w->total = o;
+    Planner p(base);
+    w->keys_in = p.take<uint64_t>(N);
+    w->keys = p.take<uint64_t>(N);
+    w->idx_in = p.take<int32_t>(N);
+    w->idx = p.take<int32_t>(N);
+    w->start = p.take<int32_t>(N + 1);  // n_com <= n for a partition with no empty component
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
 
 struct EdgesWs {
-    size_t counts, a, b, c, d, run_keys, run_count, run_start, n_pairs, n_runs, cub, total, cub_bytes;
+    int32_t* counts;
+    uint64_t* a;  // candidate keys, then the component keys
+    uint64_t* b;  // sorted candidates, then the sorted component keys
+    uint64_t* c;  // deduplicated pairs
+    uint64_t* d;  // pairs in component-key order
+    uint64_t* run_keys;
+    int32_t *run_count, *run_start, *n_pairs, *n_runs;
+    CubRegion cub;
+    size_t bytes;
 };
 
-static int plan_edges(int64_t n_tets, int64_t n_cand, EdgesWs* w) {
+static int layout(int64_t n_tets, int64_t n_cand, void* base, EdgesWs* w) {
     const int t = (int)(n_tets + 1), m = (int)(n_cand > 0 ? n_cand : 1);
-    size_t b[6] = {0, 0, 0, 0, 0, 0};
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, b[0], (const int32_t*)nullptr, (int32_t*)nullptr, t);
-    if (e == cudaSuccess)
-        e = cub::DeviceRadixSort::SortKeys(nullptr, b[1], (const uint64_t*)nullptr, (uint64_t*)nullptr, m);
-    if (e == cudaSuccess)
-        e = cub::DeviceSelect::Unique(nullptr, b[2], (const uint64_t*)nullptr, (uint64_t*)nullptr, (int32_t*)nullptr,
-                                      m);
-    if (e == cudaSuccess)
-        e = cub::DeviceRadixSort::SortPairs(nullptr, b[3], (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                            (const uint64_t*)nullptr, (uint64_t*)nullptr, m);
-    if (e == cudaSuccess)
-        e = cub::DeviceRunLengthEncode::Encode(nullptr, b[4], (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                               (int32_t*)nullptr, (int32_t*)nullptr, m);
-    if (e == cudaSuccess)
-        e = cub::DeviceScan::ExclusiveSum(nullptr, b[5], (const int32_t*)nullptr, (int32_t*)nullptr, m + 1);
-    if (e != cudaSuccess) return (int)e;
-    w->cub_bytes = 0;
-    for (size_t x : b) w->cub_bytes = x > w->cub_bytes ? x : w->cub_bytes;
+    size_t cub_bytes = 0;
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::ExclusiveSum, (const int32_t*)nullptr, (int32_t*)nullptr, t);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortKeys, (const uint64_t*)nullptr, (uint64_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceSelect::Unique, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (int32_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRadixSort::SortPairs, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (const uint64_t*)nullptr, (uint64_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceRunLengthEncode::Encode, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                  (int32_t*)nullptr, (int32_t*)nullptr, m);
+    SPG_CUB_BYTES(cub_bytes, cub::DeviceScan::ExclusiveSum, (const int32_t*)nullptr, (int32_t*)nullptr, m + 1);
     const size_t T = (size_t)t, C = n_cand > 0 ? (size_t)n_cand : 0;
-    size_t o = 0;
-    w->counts = o;     o += align256(T * 4);
-    w->a = o;          o += align256(C * 8);  // candidate keys, then the component keys
-    w->b = o;          o += align256(C * 8);  // sorted candidates, then the sorted component keys
-    w->c = o;          o += align256(C * 8);  // deduplicated pairs
-    w->d = o;          o += align256(C * 8);  // pairs in component-key order
-    w->run_keys = o;   o += align256(C * 8);
-    w->run_count = o;  o += align256((C + 1) * 4);
-    w->run_start = o;  o += align256((C + 1) * 4);
-    w->n_pairs = o;    o += 256;
-    w->n_runs = o;     o += 256;
-    w->cub = o;        o += align256(w->cub_bytes);
-    w->total = o;
+    Planner p(base);
+    w->counts = p.take<int32_t>(T);
+    w->a = p.take<uint64_t>(C);
+    w->b = p.take<uint64_t>(C);
+    w->c = p.take<uint64_t>(C);
+    w->d = p.take<uint64_t>(C);
+    w->run_keys = p.take<uint64_t>(C);
+    w->run_count = p.take<int32_t>(C + 1);
+    w->run_start = p.take<int32_t>(C + 1);
+    w->n_pairs = p.take<int32_t>(1);
+    w->n_runs = p.take<int32_t>(1);
+    w->cub = p.cub(cub_bytes);
+    w->bytes = p.bytes;
     return SPG_OK;
 }
 
-static bool too_big(int64_t n) { return n >= (1ll << 31) - 1; }
 // 12 directed pairs per tetrahedron must be countable in int32
 static bool too_many_tets(int64_t t) { return t < 0 || t > ((1ll << 31) - 2) / 12; }
 
@@ -527,61 +521,50 @@ int spg_sp_points_workspace(int64_t n, int64_t* bytes) {
     if (!bytes || n < 0) return SPG_E_BADARG;
     if (too_big(n)) return SPG_E_UNSUPPORTED;
     PointsWs w;
-    const int rc = plan_points(n, &w);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)w.total;
-    return SPG_OK;
+    const int rc = layout(n, nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_sp_points(const float* xyz, const int64_t* in_component, int64_t n, int64_t n_com, const int64_t* labels,
                   int label_mode, int64_t n_label_cols, int n_labels, void* workspace, int64_t workspace_bytes,
                   float* centroids, float* length, float* surface, float* volume, int64_t* point_count,
                   int64_t* sp_labels, uint32_t* status, spg_stream_t stream) {
-    if (n <= 0 || n_com <= 0 || n_com > n || !xyz || !in_component || !workspace || !centroids || !length ||
+    if (n <= 0 || n_com <= 0 || n_com > n || !xyz || !in_component || !centroids || !length ||
         !surface || !volume || !point_count || !status)
         return SPG_E_BADARG;
     if (label_mode < 0 || label_mode > 2 || (label_mode > 0 && (!labels || !sp_labels || n_label_cols < 1)) ||
         (label_mode == 1 && n_label_cols != (int64_t)n_labels + 1))
         return SPG_E_BADARG;
     if (too_big(n)) return SPG_E_UNSUPPORTED;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
     PointsWs w;
-    int rc = plan_points(n, &w);
+    int rc = layout(n, workspace, &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    uint64_t* keys_in = reinterpret_cast<uint64_t*>(ws + w.keys_in);
-    uint64_t* keys = reinterpret_cast<uint64_t*>(ws + w.keys);
-    int32_t* idx_in = reinterpret_cast<int32_t*>(ws + w.idx_in);
-    int32_t* idx = reinterpret_cast<int32_t*>(ws + w.idx);
-    int32_t* start = reinterpret_cast<int32_t*>(ws + w.start);
     cudaError_t e = cudaMemsetAsync(status, 0, sizeof(uint32_t), s);
     if (e == cudaSuccess && label_mode > 0)
         e = cudaMemsetAsync(sp_labels, 0, (size_t)n_com * n_label_cols * sizeof(int64_t), s);
     if (e != cudaSuccess) return (int)e;
     const unsigned blocks = (unsigned)ceil_div64(n, SPG_THREADS);
     // (y, z) first, then a stable sort by (component, x): lexicographic (component, x, y, z)
-    SPG_LAUNCH(K_SP_SORT_KEYS, s, sp_keys_lo_kernel, blocks, SPG_THREADS, 0, xyz, n, keys_in, idx_in);
-    size_t cb = w.cub_bytes;
-    e = cub::DeviceRadixSort::SortPairs(ws + w.cub, cb, (const uint64_t*)keys_in, keys, (const int32_t*)idx_in, idx,
-                                        (int)n, 0, 64, s);
-    if (e != cudaSuccess) return (int)e;
+    SPG_LAUNCH(K_SP_SORT_KEYS, s, sp_keys_lo_kernel, blocks, SPG_THREADS, 0, xyz, n, w.keys_in, w.idx_in);
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const uint64_t*)w.keys_in, w.keys, (const int32_t*)w.idx_in,
+            w.idx, (int)n, 0, 64, s);
     SPG_LAUNCH(K_SP_SORT_KEYS, s, sp_keys_hi_kernel, blocks, SPG_THREADS, 0, xyz, in_component, n,
-               (const int32_t*)idx, keys_in);
-    cb = w.cub_bytes;
-    e = cub::DeviceRadixSort::SortPairs(ws + w.cub, cb, (const uint64_t*)keys_in, keys, (const int32_t*)idx, idx_in,
-                                        (int)n, 0, 32 + id_bits(n_com), s);
-    if (e != cudaSuccess) return (int)e;
-    SPG_LAUNCH(K_SP_SORT_KEYS, s, sp_starts_kernel, blocks, SPG_THREADS, 0, (const uint64_t*)keys, n, n_com, start);
+               (const int32_t*)w.idx, w.keys_in);
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const uint64_t*)w.keys_in, w.keys, (const int32_t*)w.idx,
+            w.idx_in, (int)n, 0, 32 + id_bits(n_com), s);
+    SPG_LAUNCH(K_SP_SORT_KEYS, s, sp_starts_kernel, blocks, SPG_THREADS, 0, (const uint64_t*)w.keys, n, n_com,
+               w.start);
     PointsArgs a;
     a.xyz = xyz;
     a.labels = labels;
     a.label_mode = label_mode;
     a.n_labels = n_labels;
     a.n_label_cols = n_label_cols;
-    a.order = idx_in;
-    a.start = start;
+    a.order = w.idx_in;
+    a.start = w.start;
     a.n_com = n_com;
     a.centroids = centroids;
     a.length = length;
@@ -598,89 +581,64 @@ int spg_sp_edges_workspace(int64_t n_tets, int64_t n_cand, int64_t* bytes) {
     if (!bytes || n_tets < 0 || n_cand < 0) return SPG_E_BADARG;
     if (too_many_tets(n_tets) || n_cand > 12 * n_tets) return SPG_E_UNSUPPORTED;
     EdgesWs w;
-    const int rc = plan_edges(n_tets, n_cand, &w);
-    if (rc != SPG_OK) return rc;
-    *bytes = (int64_t)w.total;
-    return SPG_OK;
+    const int rc = layout(n_tets, n_cand, nullptr, &w);
+    if (rc == SPG_OK) *bytes = (int64_t)w.bytes;
+    return rc;
 }
 
 int spg_sp_edges_count(const int64_t* in_component, int64_t n, const void* simplices, int ids64, int64_t n_tets,
                        int32_t* tet_offsets, void* workspace, int64_t workspace_bytes, uint32_t* status,
                        spg_stream_t stream) {
-    if (n <= 0 || n_tets < 0 || !in_component || !tet_offsets || !workspace || !status || (n_tets > 0 && !simplices))
+    if (n <= 0 || n_tets < 0 || !in_component || !tet_offsets || !status || (n_tets > 0 && !simplices))
         return SPG_E_BADARG;
     if (too_big(n) || too_many_tets(n_tets)) return SPG_E_UNSUPPORTED;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
     EdgesWs w;
-    int rc = plan_edges(n_tets, 0, &w);
+    int rc = layout(n_tets, 0, workspace, &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    int32_t* counts = reinterpret_cast<int32_t*>(ws + w.counts);
     cudaError_t e = cudaMemsetAsync(status, 0, sizeof(uint32_t), s);
-    if (e == cudaSuccess) e = cudaMemsetAsync(counts + n_tets, 0, sizeof(int32_t), s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(w.counts + n_tets, 0, sizeof(int32_t), s);
     if (e != cudaSuccess) return (int)e;
     if (n_tets > 0)
         SPG_LAUNCH(K_SP_TETS, s, sp_tets_kernel<false>, (unsigned)ceil_div64(n_tets, SPG_THREADS), SPG_THREADS, 0,
-                   in_component, n, simplices, ids64, n_tets, counts, (const int32_t*)nullptr, (uint64_t*)nullptr,
+                   in_component, n, simplices, ids64, n_tets, w.counts, (const int32_t*)nullptr, (uint64_t*)nullptr,
                    (unsigned*)status);
-    size_t cb = w.cub_bytes;
-    e = cub::DeviceScan::ExclusiveSum(ws + w.cub, cb, (const int32_t*)counts, tet_offsets, (int)n_tets + 1, s);
-    if (e != cudaSuccess) return (int)e;
+    SPG_CUB(w.cub, cub::DeviceScan::ExclusiveSum, (const int32_t*)w.counts, tet_offsets, (int)n_tets + 1, s);
     return launch_status();
 }
 
 int spg_sp_edges_build(const float* xyz, const int64_t* in_component, int64_t n, const void* simplices, int ids64,
                        int64_t n_tets, const int32_t* tet_offsets, int64_t n_cand, double d_max, void* workspace,
                        int64_t workspace_bytes, int64_t* n_sedg, spg_stream_t stream) {
-    if (n <= 0 || n_tets < 0 || n_cand < 0 || !xyz || !in_component || !tet_offsets || !workspace || !n_sedg ||
+    if (n <= 0 || n_tets < 0 || n_cand < 0 || !xyz || !in_component || !tet_offsets || !n_sedg ||
         (n_tets > 0 && !simplices))
         return SPG_E_BADARG;
     if (too_big(n) || too_many_tets(n_tets) || n_cand > 12 * n_tets) return SPG_E_UNSUPPORTED;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return SPG_E_ALIGN;
     EdgesWs w;
-    int rc = plan_edges(n_tets, n_cand, &w);
+    int rc = layout(n_tets, n_cand, workspace, &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
     cudaStream_t s = (cudaStream_t)stream;
     if (n_cand == 0) return (int)cudaMemsetAsync(n_sedg, 0, sizeof(int64_t), s);
-    uint8_t* ws = static_cast<uint8_t*>(workspace);
-    uint64_t* A = reinterpret_cast<uint64_t*>(ws + w.a);
-    uint64_t* B = reinterpret_cast<uint64_t*>(ws + w.b);
-    uint64_t* C = reinterpret_cast<uint64_t*>(ws + w.c);
-    uint64_t* D = reinterpret_cast<uint64_t*>(ws + w.d);
-    uint64_t* run_keys = reinterpret_cast<uint64_t*>(ws + w.run_keys);
-    int32_t* run_count = reinterpret_cast<int32_t*>(ws + w.run_count);
-    int32_t* run_start = reinterpret_cast<int32_t*>(ws + w.run_start);
-    int32_t* n_pairs = reinterpret_cast<int32_t*>(ws + w.n_pairs);
-    int32_t* n_runs = reinterpret_cast<int32_t*>(ws + w.n_runs);
     const int m = (int)n_cand;
     SPG_LAUNCH(K_SP_TETS, s, sp_tets_kernel<true>, (unsigned)ceil_div64(n_tets, SPG_THREADS), SPG_THREADS, 0,
-               in_component, n, simplices, ids64, n_tets, (int32_t*)nullptr, tet_offsets, A, (unsigned*)nullptr);
+               in_component, n, simplices, ids64, n_tets, (int32_t*)nullptr, tet_offsets, w.a, (unsigned*)nullptr);
     const int bits = id_bits(n);
-    size_t cb = w.cub_bytes;
-    cudaError_t e = cub::DeviceRadixSort::SortKeys(ws + w.cub, cb, (const uint64_t*)A, B, m, 0, 32 + bits, s);
-    if (e != cudaSuccess) return (int)e;
-    cb = w.cub_bytes;
-    e = cub::DeviceSelect::Unique(ws + w.cub, cb, (const uint64_t*)B, C, n_pairs, m, s);
-    if (e != cudaSuccess) return (int)e;
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortKeys, (const uint64_t*)w.a, w.b, m, 0, 32 + bits, s);
+    SPG_CUB(w.cub, cub::DeviceSelect::Unique, (const uint64_t*)w.b, w.c, w.n_pairs, m, s);
     SPG_LAUNCH(K_SP_PAIRS, s, sp_pairs_kernel, (unsigned)ceil_div64(n_cand, SPG_THREADS), SPG_THREADS, 0, xyz,
-               in_component, (const uint64_t*)C, (const int32_t*)n_pairs, n_cand, d_max, A);
+               in_component, (const uint64_t*)w.c, (const int32_t*)w.n_pairs, n_cand, d_max, w.a);
     // the dropped pairs (key ~0) sort last; the component ids are below 2^31, so all 64 bits are sorted
-    cb = w.cub_bytes;
-    e = cub::DeviceRadixSort::SortPairs(ws + w.cub, cb, (const uint64_t*)A, B, (const uint64_t*)C, D, m, 0, 64, s);
-    if (e != cudaSuccess) return (int)e;
+    SPG_CUB(w.cub, cub::DeviceRadixSort::SortPairs, (const uint64_t*)w.a, w.b, (const uint64_t*)w.c, w.d, m, 0, 64,
+            s);
     // counts beyond the last run stay 0, so the scan is valid for every run
-    e = cudaMemsetAsync(run_count, 0, ((size_t)m + 1) * 4, s);
+    const cudaError_t e = cudaMemsetAsync(w.run_count, 0, ((size_t)m + 1) * 4, s);
     if (e != cudaSuccess) return (int)e;
-    cb = w.cub_bytes;
-    e = cub::DeviceRunLengthEncode::Encode(ws + w.cub, cb, (const uint64_t*)B, run_keys, run_count, n_runs, m, s);
-    if (e != cudaSuccess) return (int)e;
-    cb = w.cub_bytes;
-    e = cub::DeviceScan::ExclusiveSum(ws + w.cub, cb, (const int32_t*)run_count, run_start, m + 1, s);
-    if (e != cudaSuccess) return (int)e;
-    SPG_LAUNCH(K_SP_PAIRS, s, sp_count_kernel, 1, 1, 0, (const uint64_t*)run_keys, (const int32_t*)n_runs, n_sedg);
+    SPG_CUB(w.cub, cub::DeviceRunLengthEncode::Encode, (const uint64_t*)w.b, w.run_keys, w.run_count, w.n_runs, m, s);
+    SPG_CUB(w.cub, cub::DeviceScan::ExclusiveSum, (const int32_t*)w.run_count, w.run_start, m + 1, s);
+    SPG_LAUNCH(K_SP_PAIRS, s, sp_count_kernel, 1, 1, 0, (const uint64_t*)w.run_keys, (const int32_t*)w.n_runs,
+               n_sedg);
     return launch_status();
 }
 
@@ -698,16 +656,15 @@ int spg_sp_edges_features(const float* xyz, int64_t n_tets, int64_t n_cand, cons
         return SPG_E_BADARG;
     if (too_many_tets(n_tets) || n_cand > 12 * n_tets) return SPG_E_UNSUPPORTED;
     EdgesWs w;
-    const int rc = plan_edges(n_tets, n_cand, &w);
+    int rc = layout(n_tets, n_cand, const_cast<void*>(workspace), &w);
+    if (rc == SPG_OK) rc = ws_check(workspace, workspace_bytes, w.bytes);
     if (rc != SPG_OK) return rc;
-    if (workspace_bytes < (int64_t)w.total) return SPG_E_BADARG;
-    const uint8_t* ws = static_cast<const uint8_t*>(workspace);
     EdgesArgs a;
     a.xyz = xyz;
-    a.pairs = reinterpret_cast<const uint64_t*>(ws + w.d);
-    a.run_keys = reinterpret_cast<const uint64_t*>(ws + w.run_keys);
-    a.run_start = reinterpret_cast<const int32_t*>(ws + w.run_start);
-    a.run_count = reinterpret_cast<const int32_t*>(ws + w.run_count);
+    a.pairs = w.d;
+    a.run_keys = w.run_keys;
+    a.run_start = w.run_start;
+    a.run_count = w.run_count;
     a.n_sedg = n_sedg;
     a.centroids = centroids;
     a.length = length;

@@ -57,6 +57,14 @@ def workspace(nfloats, device, slot=0):
     return buf
 
 
+def _workspace(query, device, *sizes):
+    """uint8 scratch of the bytes that the C-ABI query `query` reports for `sizes` (torch's allocations are
+    256-byte aligned, as the entry points require)."""
+    nbytes = torch.zeros(1, dtype=torch.int64)
+    _lib.call(query, *[int(n) for n in sizes], nbytes)
+    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
+
+
 WEIGHTS_GENERATION = [0]
 
 
@@ -145,13 +153,11 @@ class EccGraph(object):
 def graph_build_alloc(n_out, n_in, n_edges, device):
     """Output tensors + status word + workspace of spg_graph_build (static addresses: a captured CUDA graph
     reads them, HostBatch.copy_into rebuilds into them)."""
-    nbytes = torch.zeros(1, dtype=torch.int64)
-    _lib.call("spg_graph_build_workspace", n_out, n_in, n_edges, nbytes)
     i32 = dict(dtype=torch.int32, device=device)
     return {"tgt_rowptr": torch.empty(n_out + 1, **i32), "idxn": torch.empty(n_edges, **i32),
             "edge_tgt": torch.empty(n_edges, **i32), "src_rowptr": torch.empty(n_in + 1, **i32),
             "src_perm": torch.empty(n_edges, **i32), "idxe": None, "status": torch.zeros(1, **i32),
-            "_ws": torch.empty(int(nbytes[0]) + 256, dtype=torch.uint8, device=device)}
+            "_ws": _workspace("spg_graph_build_workspace", device, n_out, n_in, n_edges)}
 
 
 def graph_build_into(dev, idxn, degs, n_in):
@@ -159,10 +165,9 @@ def graph_build_into(dev, idxn, degs, n_in):
     _need_cuda(idxn, degs)
     assert idxn.dtype == torch.int64 and degs.dtype == torch.int64 and idxn.is_contiguous() and degs.is_contiguous()
     ws = dev["_ws"]
-    off = (-ws.data_ptr()) % 256
     _lib.call("spg_graph_build", idxn, degs, degs.numel(), int(n_in), idxn.numel(), dev["idxn"], dev["tgt_rowptr"],
-              dev["edge_tgt"], dev["src_rowptr"], dev["src_perm"], dev["status"], ws.data_ptr() + off,
-              ws.numel() - off, _lib.current_stream())
+              dev["edge_tgt"], dev["src_rowptr"], dev["src_perm"], dev["status"], ws, ws.numel(),
+              _lib.current_stream())
 
 
 def build_csr_host(idxn, degs, n_in):
@@ -1218,13 +1223,6 @@ LP_INTRA = {"tv": 0, "laplacian": 1, "TVH": 2}
 LP_INTER = {None: -1, "zhang": 0, "TVminus": 1}
 
 
-def _lp_sort_ws(n, dev):
-    nbytes = torch.zeros(1, dtype=torch.int64)
-    _lib.call("spg_lp_sort_workspace", int(n), nbytes)
-    ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=dev)
-    return ws, ws.numel()
-
-
 def lp_incidence(src, tgt, n_ver):
     """Per-vertex CSR of the edge endpoints: (rowptr int32 [V+1], entry int32 [2E]); entry j < E is the source
     side of edge j, j >= E the target side of edge j - E."""
@@ -1232,9 +1230,8 @@ def lp_incidence(src, tgt, n_ver):
     dev, E = src.device, src.numel()
     i32 = dict(dtype=torch.int32, device=dev)
     rowptr, entry = torch.empty(n_ver + 1, **i32), torch.empty(2 * E, **i32)
-    k0, k1, v0 = torch.empty(2 * E, **i32), torch.empty(2 * E, **i32), torch.empty(2 * E, **i32)
-    ws, nb = _lp_sort_ws(2 * E, dev)
-    _lib.call("spg_lp_incidence", src, tgt, n_ver, E, rowptr, entry, k0, k1, v0, ws, nb, _lib.current_stream())
+    ws = _workspace("spg_lp_workspace", dev, n_ver, E, 0)
+    _lib.call("spg_lp_incidence", src, tgt, n_ver, E, rowptr, entry, ws, ws.numel(), _lib.current_stream())
     return rowptr, entry
 
 
@@ -1288,13 +1285,9 @@ def lp_xpart(src, tgt, is_transition, pred_in_component, n_ver, transition_facto
     i32 = dict(dtype=torch.int32, device=dev)
     w = torch.empty(E, dtype=torch.float32, device=dev)
     inx, size, ncomp = torch.empty(n_ver, **i32), torch.empty(n_ver, **i32), torch.empty(1, **i32)
-    par, root, rank = torch.empty(n_ver, **i32), torch.empty(n_ver, **i32), torch.empty(n_ver, **i32)
-    k0 = torch.empty(E, dtype=torch.int64, device=dev)
-    k1 = torch.empty(E, dtype=torch.int64, device=dev)
-    v0, v1 = torch.empty(E, **i32), torch.empty(E, **i32)
-    ws, nb = _lp_sort_ws(max(n_ver, E), dev)
+    ws = _workspace("spg_lp_workspace", dev, n_ver, E, 0)
     _lib.call("spg_lp_xpart", src, tgt, is_transition, pred_in_component, n_ver, E, float(transition_factor), w, inx,
-              size, ncomp, par, root, rank, k0, k1, v0, v1, ws, nb, _lib.current_stream())
+              size, ncomp, ws, ws.numel(), _lib.current_stream())
     return w, inx, size, ncomp
 
 
@@ -1302,13 +1295,10 @@ def lp_seal(src, tgt, is_transition, pred_in_component, objects, n_comp, transit
     """SEAL weights: (weights float32 [E], w_per_component int32 [n_comp])."""
     _need_cuda(src, tgt, is_transition, pred_in_component, objects)
     dev, E, V = src.device, src.numel(), pred_in_component.numel()
-    i32 = dict(dtype=torch.int32, device=dev)
-    w, wc = torch.empty(E, dtype=torch.float32, device=dev), torch.empty(n_comp, **i32)
-    st, mt = torch.empty(n_comp, **i32), torch.empty(n_comp, **i32)
-    k0, k1 = torch.empty(V, dtype=torch.int64, device=dev), torch.empty(V, dtype=torch.int64, device=dev)
-    ws, nb = _lp_sort_ws(V, dev)
+    w, wc = torch.empty(E, dtype=torch.float32, device=dev), torch.empty(n_comp, dtype=torch.int32, device=dev)
+    ws = _workspace("spg_lp_workspace", dev, V, E, n_comp)
     _lib.call("spg_lp_seal", src, tgt, is_transition, pred_in_component, objects, V, E, n_comp,
-              float(transition_factor), w, wc, st, mt, k0, k1, ws, nb, _lib.current_stream())
+              float(transition_factor), w, wc, ws, ws.numel(), _lib.current_stream())
     return w, wc
 
 
@@ -1380,14 +1370,9 @@ def lp_subgraph_select(mask, objects, src, tgt, new_index, selected, edge_pos, o
     spg_lp_subgraph_select."""
     _need_cuda(mask, objects, src, tgt, new_index, selected, edge_pos, object_max)
     n, E = objects.numel(), src.numel()
-    ws, nb = None, 0
-    if mask is not None:
-        nbytes = torch.zeros(1, dtype=torch.int64)
-        _lib.call("spg_lp_subgraph_workspace", n, E, nbytes)
-        ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=objects.device)
-        nb = ws.numel()
+    ws = None if mask is None else _workspace("spg_lp_subgraph_workspace", objects.device, n, E)
     _lib.call("spg_lp_subgraph_select", mask, objects, n, src, tgt, E, new_index, selected, edge_pos, object_max, ws,
-              nb, _lib.current_stream())
+              0 if ws is None else ws.numel(), _lib.current_stream())
 
 
 def lp_subgraph_edges(src, tgt, is_transition, new_index, edge_pos, vertex_offset, src_out, tgt_out, tr_out):
@@ -1432,9 +1417,7 @@ def knn_bounds(xyz):
 
 
 def knn_workspace(n, device):
-    nbytes = torch.zeros(1, dtype=torch.int64)
-    _lib.call("spg_knn_workspace", int(n), nbytes)
-    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
+    return _workspace("spg_knn_workspace", device, n)
 
 
 def knn_grid(xyz, grid, ws):
@@ -1494,9 +1477,7 @@ def sp_points(xyz, in_component, n_com, labels, label_mode, n_labels):
     _need_cuda(xyz, in_component, labels)
     assert in_component.dtype == torch.int64 and in_component.is_contiguous()
     dev, n = xyz.device, xyz.shape[0]
-    nbytes = torch.zeros(1, dtype=torch.int64)
-    _lib.call("spg_sp_points_workspace", int(n), nbytes)
-    ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=dev)
+    ws = _workspace("spg_sp_points_workspace", dev, n)
     cols = 0
     if label_mode:
         assert labels.dtype == torch.int64 and labels.is_contiguous()
@@ -1511,19 +1492,13 @@ def sp_points(xyz, in_component, n_com, labels, label_mode, n_labels):
     return (cen, f[0], f[1], f[2], count, sp_labels), status
 
 
-def _edges_workspace(n_tets, n_cand, device):
-    nbytes = torch.zeros(1, dtype=torch.int64)
-    _lib.call("spg_sp_edges_workspace", int(n_tets), int(n_cand), nbytes)
-    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
-
-
 def sp_edges_count(in_component, simplices):
     """(tet_offsets int32 [T + 1], status int32 [1]; 2: an id outside [0, n)) on the device for simplices int32 or
     int64 [T, 4]; tet_offsets[T] is the number of candidate pairs.  See spg_sp_edges_count."""
     _need_cuda(in_component, simplices)
     assert simplices.dtype in (torch.int32, torch.int64) and simplices.is_contiguous()
     dev, t = in_component.device, simplices.shape[0]
-    ws = _edges_workspace(t, 0, dev)
+    ws = _workspace("spg_sp_edges_workspace", dev, t, 0)
     offsets = torch.empty(t + 1, dtype=torch.int32, device=dev)
     status = torch.empty(1, dtype=torch.int32, device=dev)
     _lib.call("spg_sp_edges_count", in_component, in_component.shape[0], simplices,
@@ -1536,7 +1511,7 @@ def sp_edges_build(xyz, in_component, simplices, offsets, n_cand, d_max):
     spg_sp_edges_build."""
     _need_cuda(xyz, in_component, simplices, offsets)
     dev, t = xyz.device, simplices.shape[0]
-    ws = _edges_workspace(t, n_cand, dev)
+    ws = _workspace("spg_sp_edges_workspace", dev, t, n_cand)
     n_sedg = torch.empty(1, dtype=torch.int64, device=dev)
     _lib.call("spg_sp_edges_build", xyz, in_component, xyz.shape[0], simplices, int(simplices.dtype == torch.int64),
               int(t), offsets, int(n_cand), float(d_max), ws, ws.numel(), n_sedg, _lib.current_stream())
@@ -1566,9 +1541,7 @@ def sp_edges_features(xyz, n_tets, n_cand, ws, n_sedg, sp):
 
 # ------------------------------------------------------------- voxel pruning
 def prune_workspace(n, chunk_rows, device):
-    nbytes = torch.zeros(1, dtype=torch.int64)
-    _lib.call("spg_prune_workspace", int(n), int(chunk_rows), nbytes)
-    return torch.empty(int(nbytes[0]), dtype=torch.uint8, device=device)
+    return _workspace("spg_prune_workspace", device, n, chunk_rows)
 
 
 def prune_bounds(xyz, chunk_rows, voxel_size, labels, n_labels, objects, n_objects, ws):

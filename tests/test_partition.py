@@ -134,9 +134,9 @@ def test_loss_kinds_follow_the_reference_order():
         assert pref.loss_kinds(name) == loss_kinds(name), name
 
 
-def test_abi_symbols_and_kernel_names():
+def test_abi_symbols_and_kernel_names_with_one_lp_workspace_query():
     from superpoint_graph_b200 import _lib
-    names = ["spg_lp_sort_workspace", "spg_lp_incidence", "spg_lp_dist_fwd", "spg_lp_dist_bwd",
+    names = ["spg_lp_workspace", "spg_lp_incidence", "spg_lp_dist_fwd", "spg_lp_dist_bwd",
              "spg_lp_loss_partials", "spg_lp_loss_fwd", "spg_lp_loss_bwd", "spg_lp_xpart", "spg_lp_seal",
              "spg_lp_fill_weights", "spg_lp_count", "spg_lp_edge_weight", "spg_lp_relax",
              "spg_lp_perfect_prediction"]
