@@ -828,6 +828,56 @@ int spg_prune_reduce(const float* xyz, const uint8_t* rgb, const int64_t* labels
                      int64_t workspace_bytes, int64_t n_voxels, float* xyz_out, uint8_t* rgb_out,
                      int64_t* labels_out, int64_t* objects_out, spg_stream_t stream);
 
+/* ---------------------------------------------------------------- cut pursuit
+ * libcp.cutpursuit of both partition pipelines (ref: partition/cut-pursuit/src/cutpursuit.cpp:77-105, speed 4;
+ * spatial 0: CutPursuit_L2, 1: CutPursuit_SPG), one stage per call; spg_cut_pursuit.py runs the main loop.
+ * n vertices, n_edges listed edges (each one an arc pair, duplicates kept), dim in [1, 32], 2 n_edges < 2^31 - 1.
+ * One workspace of spg_cp_workspace(n, n_edges, dim) bytes (256-byte aligned) holds the whole state; every call
+ * takes the same (n, n_edges, dim, workspace).  spg_cp_regions writes the byte offsets in the workspace of: obs,
+ * comp (int32 [n]), root (int32), sat (uint8), label (uint8), colour (uint8: 0 source tree, 1 free, 4 sink tree),
+ * active (uint8 [n_edges]), value, c0, c1 (float64 [n, dim]), cs, ct (float32 [n]), ecap (float32 [n_edges]),
+ * members, offsets (int32), words (int64), dwords (float64), partner (int32 [n]), res (int64 [2 n_edges]: the
+ * residual fixed-point capacities of the arcs), excess, rt (int64 [n]: excess and residual sink capacity), arc_off
+ * (int32 [n + 1]), arc_dst, arc_rev, arc_edge (int32 [2 n_edges]: head, reverse arc and listed edge of every arc).
+ *
+ * spg_cp_setup: out[0] (host) = status (1: a non-finite observation, 2: a non-finite edge weight, 4: an edge id
+ *   outside [0, n)); when 0, the arc CSR, one component (root 0, its mean as value), no active edge.
+ * spg_cp_members: members / offsets = the vertices grouped by component, ascending.
+ * spg_cp_kmeans: labels = 0, then 2-means per unsaturated component of >= 2 vertices (members current).
+ * spg_cp_centers: c0 / c1 of every unsaturated component; L2 saturates a component with an empty side.
+ * spg_cp_capacities: cs / ct / ecap, the reference's fp32 capacities (unary: the SPG step's weight).
+ * spg_cp_maxflow: colour and labels from the minimal cuts; out[0] = push-relabel rounds.
+ * spg_cp_activate: L2 saturation, edge activation; out[0] = vertices in saturated components.
+ * spg_cp_split: the connected components of the non-active graph; out[0] = the new component count.
+ * spg_cp_merge: one merge pass (is_cutoff: merge(true)); out[0] = merges, out[1] = the new component count.
+ * spg_cp_energy: out[0..2] (host) = fidelity, active edge weight, fidelity + reg_strength * weight.
+ * spg_cp_output: in_component [n], offsets [n_comp + 1], members [n] (device, int64).                      */
+int spg_cp_workspace(int64_t n, int64_t n_edges, int dim, int64_t* bytes);
+int spg_cp_regions(int64_t n, int64_t n_edges, int dim, int64_t* offsets);
+int spg_cp_setup(const float* obs, const int64_t* source, const int64_t* target, const float* edge_weight,
+                 int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t* out,
+                 spg_stream_t stream);
+int spg_cp_members(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                   spg_stream_t stream);
+int spg_cp_kmeans(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                  int64_t iteration, int64_t seed, spg_stream_t stream);
+int spg_cp_centers(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                   int spatial, spg_stream_t stream);
+int spg_cp_capacities(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes,
+                      float reg_strength, float unary, int spatial, spg_stream_t stream);
+int spg_cp_maxflow(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t* out,
+                   spg_stream_t stream);
+int spg_cp_activate(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                    int spatial, int64_t* out, spg_stream_t stream);
+int spg_cp_split(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                 int64_t* out, spg_stream_t stream);
+int spg_cp_merge(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                 double reg_strength, double cutoff, int is_cutoff, int64_t* out, spg_stream_t stream);
+int spg_cp_energy(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes,
+                  double reg_strength, double* out, spg_stream_t stream);
+int spg_cp_output(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
+                  int64_t* in_component, int64_t* offsets, int64_t* members, spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

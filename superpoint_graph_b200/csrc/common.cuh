@@ -93,6 +93,17 @@ enum KernelId {
     K_PRUNE_KEYS,
     K_PRUNE_ROWS,
     K_PRUNE_REDUCE,
+    K_CP_GRAPH,
+    K_CP_MEMBERS,
+    K_CP_KMEANS,
+    K_CP_CENTERS,
+    K_CP_CAPACITIES,
+    K_CP_MAXFLOW,
+    K_CP_COLOUR,
+    K_CP_ACTIVATE,
+    K_CP_SPLIT,
+    K_CP_MERGE,
+    K_CP_ENERGY,
     K_COUNT
 };
 

@@ -34,6 +34,9 @@ static const char* kKernelNames[K_COUNT] = {
     "sp_scan",           "sp_sort_keys",       "sp_points",           "sp_tets",
     "sp_pairs",          "sp_edges",
     "prune_bounds",      "prune_keys",         "prune_rows",          "prune_reduce",
+    "cp_graph",          "cp_members",         "cp_kmeans",           "cp_centers",
+    "cp_capacities",     "cp_maxflow",         "cp_colour",           "cp_activate",
+    "cp_split",          "cp_merge",           "cp_energy",
 };
 
 struct Record {

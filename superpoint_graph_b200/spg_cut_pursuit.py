@@ -1,0 +1,304 @@
+"""The l0 cut pursuit partition on the device: `libcp.cutpursuit` of both partition pipelines (ref:
+partition/cut-pursuit/src/cutpursuit.cpp:77-105; called at partition/partition.py:177 and
+supervized_partition/losses.py:82).
+
+    from superpoint_graph_b200.spg_cut_pursuit import cutpursuit, to_numpy
+
+    components, in_component = cutpursuit(features, source, target, edge_weight, reg_strength)
+    graph_sp = compute_sp_graph(xyz, d_max, in_component, components, labels, n_labels)
+
+Same arguments as libcp (speed 4: 3 flow steps, 10 k-means restarts of 5 iterations, at most 15 iterations, a
+backward merge step, stopping ratio 0.05; every vertex weighs 1).  spatial = 0 is CutPursuit_L2, 1 is
+CutPursuit_SPG.  in_component is an int64 CUDA tensor and components a `Components` CSR value (len() and indexing);
+to_numpy gives libcp's types.  The k-means draws are Philox4x32-10 keyed by `seed`, so a partition is reproducible;
+the minimal-cut colouring, the component numbering and the merge selection are the reference's (DESIGN.md §4).
+The kernels are in csrc/cut_pursuit.cu.
+"""
+import math
+
+import numpy as np
+import torch
+
+from . import _lib, ops
+
+__all__ = ["Components", "cutpursuit", "to_numpy", "compute_partition"]
+
+FLOW_STEPS, MAX_ITE_MAIN, STOPPING_RATIO, CUTOFF_ROUNDS = 3, 15, 0.05, 50
+REGIONS = ("obs", "comp", "root", "sat", "label", "colour", "active", "value", "c0", "c1", "cs", "ct", "ecap",
+           "members", "offsets", "words", "dwords", "partner", "res", "excess", "rt", "arc_off", "arc_dst", "arc_rev",
+           "arc_edge")
+
+
+class Components:
+    """The components of a partition as a CSR: offsets [n_com + 1] and members [n] (int64 CUDA, ascending vertex
+    id within a component).  len() is the component count; components[i] is the members of component i."""
+
+    def __init__(self, offsets, members):
+        self.offsets = offsets
+        self.members = members
+        self._host = None
+
+    def __len__(self):
+        return self.offsets.numel() - 1
+
+    def __getitem__(self, i):
+        if self._host is None:
+            self._host = self.offsets.cpu().numpy()
+        n = len(self)
+        if i < 0:
+            i += n
+        if not 0 <= i < n:
+            raise IndexError("component %d out of range for %d components" % (i, n))
+        return self.members[int(self._host[i]):int(self._host[i + 1])]
+
+
+def unary_weights(weight_decay):
+    """SPG's per-step weights (CutPursuit_SPG.h:75-79): float32 decay^-3, then times decay before each step."""
+    wd = np.float32(weight_decay)
+    u = np.float32(np.power(wd, np.float32(-FLOW_STEPS)))
+    out = []
+    for _ in range(FLOW_STEPS):
+        u = np.float32(u * wd)
+        out.append(float(u))
+    return out
+
+
+def _device(*xs):
+    for x in xs:
+        if torch.is_tensor(x) and x.is_cuda:
+            return x.device
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _float32(a, name, dev):
+    if torch.is_tensor(a):
+        if a.dtype != torch.float32:
+            raise TypeError("%s must be float32 (got %s)" % (name, a.dtype))
+        return a.detach().to(dev).contiguous()
+    a = np.asarray(a)
+    if a.dtype != np.float32:
+        raise TypeError("%s must be float32 (got %s)" % (name, a.dtype))
+    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+
+
+def _ids(a, name, dev):
+    if torch.is_tensor(a):
+        if a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
+            raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
+        return a.detach().to(device=dev, dtype=torch.int64).reshape(-1).contiguous()
+    a = np.asarray(a)
+    if a.dtype.kind not in "iu":
+        raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
+    return torch.from_numpy(np.ascontiguousarray(a.reshape(-1), dtype=np.int64)).to(dev)
+
+
+class State:
+    """The device state of one cut pursuit: the workspace and the stage calls on it (csrc/cut_pursuit.cu)."""
+
+    def __init__(self, obs, source, target, edge_weight):
+        self.n, self.D = obs.shape
+        self.E = source.numel()
+        self.dev = obs.device
+        self.ws = ops._workspace("spg_cp_workspace", self.dev, self.n, self.E, self.D)
+        self.out = torch.zeros(4, dtype=torch.int64)
+        self.dout = torch.zeros(4, dtype=torch.float64)
+        self._call("spg_cp_setup", obs, source, target, edge_weight, *self._dims(), self.out)
+        self.status = int(self.out[0])
+        self.n_comp = 1
+
+    def _dims(self):
+        return self.n, self.E, self.D, self.ws, self.ws.numel()
+
+    def _call(self, name, *args):
+        _lib.call(name, *args, _lib.current_stream())
+
+    def region(self, name, dtype, count):
+        offs = torch.zeros(len(REGIONS), dtype=torch.int64)
+        _lib.call("spg_cp_regions", self.n, self.E, self.D, offs)
+        o = int(offs[REGIONS.index(name)])
+        nb = torch.empty((), dtype=dtype).element_size() * count
+        return self.ws[o:o + nb].view(dtype)
+
+    def members(self):
+        self._call("spg_cp_members", *self._dims(), self.n_comp)
+
+    def kmeans(self, iteration, seed):
+        self._call("spg_cp_kmeans", *self._dims(), self.n_comp, int(iteration), int(seed))
+
+    def centers(self, spatial):
+        self._call("spg_cp_centers", *self._dims(), self.n_comp, int(spatial))
+
+    def capacities(self, reg_strength, unary, spatial):
+        self._call("spg_cp_capacities", *self._dims(), float(reg_strength), float(unary), int(spatial))
+
+    def maxflow(self):
+        self._call("spg_cp_maxflow", *self._dims(), self.out)
+        return int(self.out[0])
+
+    def activate(self, spatial):
+        self._call("spg_cp_activate", *self._dims(), self.n_comp, int(spatial), self.out)
+        return int(self.out[0])
+
+    def split(self):
+        self._call("spg_cp_split", *self._dims(), self.n_comp, self.out)
+        self.n_comp = int(self.out[0])
+
+    def merge(self, reg_strength, cutoff, is_cutoff):
+        self._call("spg_cp_merge", *self._dims(), self.n_comp, float(reg_strength), float(cutoff), int(is_cutoff),
+                   self.out)
+        self.n_comp = int(self.out[1])
+        return int(self.out[0])
+
+    def energy(self, reg_strength):
+        self._call("spg_cp_energy", *self._dims(), float(reg_strength), self.dout)
+        return float(self.dout[2])
+
+    def output(self):
+        in_component = torch.empty(self.n, dtype=torch.int64, device=self.dev)
+        offsets = torch.empty(self.n_comp + 1, dtype=torch.int64, device=self.dev)
+        members = torch.empty(self.n, dtype=torch.int64, device=self.dev)
+        self._call("spg_cp_output", *self._dims(), self.n_comp, in_component, offsets, members)
+        return Components(offsets, members), in_component
+
+
+def _relative_drop(old, new):
+    """(old - new) / old with IEEE semantics (a zero old energy gives nan or +-inf, never an exception)."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return float(np.float64(old - new) / np.float64(old))
+
+
+def run(state, reg_strength, cutoff, spatial, weight_decay, seed, timer=None, stats=None):
+    """CutPursuit::run (ref: CutPursuit.h:73-160) on a set-up State; `timer(stage)` brackets each stage when
+    given, and `stats` collects the iteration count and the push-relabel rounds."""
+    lam = float(np.float32(reg_strength))
+    unary = unary_weights(weight_decay) if spatial else [1.0] * FLOW_STEPS
+    tick = timer or (lambda stage: _Null())
+    old = state.energy(lam)
+    ite = rounds = 0
+    for ite in range(1, MAX_ITE_MAIN + 1):
+        with tick("kmeans"):
+            state.members()
+            state.kmeans(ite, seed)
+        for step in range(FLOW_STEPS):
+            with tick("flow"):
+                state.centers(spatial)
+                state.capacities(lam, unary[step], spatial)
+                rounds += state.maxflow()
+        with tick("colour"):
+            saturation = state.activate(spatial)
+        with tick("split"):
+            state.split()
+        with tick("merge"):
+            state.merge(lam, 0, False)
+        energy = state.energy(lam)
+        if saturation == state.n:
+            break
+        if _relative_drop(old, energy) < STOPPING_RATIO:
+            break
+        old = energy
+    if cutoff > 0:
+        with tick("cutoff"):
+            i = 0
+            while True:
+                n_merged = state.merge(lam, cutoff, True)
+                i += 1
+                if n_merged == 0 or i > CUTOFF_ROUNDS:
+                    break
+    if stats is not None:
+        stats.update(iterations=ite, push_relabel_rounds=rounds, components=state.n_comp,
+                     energy=state.energy(lam))
+
+
+class _Null:
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        return False
+
+
+def prepare(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial=0, weight_decay=1.0):
+    """Host validation and the device state; see cutpursuit."""
+    shape = tuple(obs.shape)
+    if len(shape) != 2 or shape[0] < 1:
+        raise ValueError("obs must be [n, D] with n >= 1 (got shape %s)" % (shape,))
+    n, D = shape
+    if not 1 <= D <= 32:
+        raise ValueError("obs must have between 1 and 32 columns (got %d)" % D)
+    if cutoff < 0:
+        raise ValueError("cutoff must be >= 0 (got %r)" % (cutoff,))
+    if spatial not in (0, 1):
+        raise ValueError("spatial must be 0 or 1 (got %r)" % (spatial,))
+    if not weight_decay > 0:
+        raise ValueError("weight_decay must be > 0 (got %r)" % (weight_decay,))
+    if not math.isfinite(float(reg_strength)):
+        raise ValueError("reg_strength must be finite (got %r)" % (reg_strength,))
+    for a, name in ((obs, "obs"), (edge_weight, "edge_weight")):
+        dt = a.dtype if torch.is_tensor(a) else np.asarray(a).dtype
+        if dt not in (torch.float32, np.float32):
+            raise TypeError("%s must be float32 (got %s)" % (name, dt))
+    for a, name in ((source, "source"), (target, "target")):
+        if torch.is_tensor(a):
+            if a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
+                raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
+        elif np.asarray(a).dtype.kind not in "iu":
+            raise TypeError("%s must hold integers (got %s)" % (name, np.asarray(a).dtype))
+    sizes = [a.numel() if torch.is_tensor(a) else np.asarray(a).size for a in (source, target, edge_weight)]
+    if len(set(sizes)) != 1:
+        raise ValueError("source, target and edge_weight must have one entry per edge (got %d, %d, %d)"
+                         % tuple(sizes))
+    dev = _device(obs, source, target, edge_weight)
+    obs_t = _float32(obs, "obs", dev)
+    w = _float32(edge_weight, "edge_weight", dev).reshape(-1)
+    src = _ids(source, "source", dev)
+    tgt = _ids(target, "target", dev)
+    with torch.cuda.device(dev):
+        state = State(obs_t, src, tgt, w)
+    if state.status & 4:
+        raise IndexError("an edge id is outside [0, %d)" % n)
+    if state.status & 1:
+        raise ValueError("obs contains NaN or infinity")
+    if state.status & 2:
+        raise ValueError("edge_weight contains NaN or infinity")
+    return state
+
+
+def cutpursuit(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial=0, weight_decay=1.0, seed=0):
+    """(components, in_component) of the l0 cut pursuit partition of obs on the graph (source, target,
+    edge_weight) (ref: libcp.cutpursuit).
+
+    TypeError: obs or edge_weight not float32, non-integer ids.  ValueError: shapes, D outside [1, 32], cutoff < 0,
+    spatial not in {0, 1}, weight_decay <= 0, non-finite observations or weights.  IndexError: an edge id outside
+    [0, n)."""
+    state = prepare(obs, source, target, edge_weight, reg_strength, cutoff, spatial, weight_decay)
+    with torch.cuda.device(state.dev):
+        run(state, reg_strength, cutoff, spatial, weight_decay, seed)
+        return state.output()
+
+
+def to_numpy(partition):
+    """libcp's types: a list of uint32 member arrays and a uint32 in_component."""
+    components, in_component = partition
+    off = components.offsets.cpu().numpy()
+    mem = components.members.cpu().numpy().astype(np.uint32)
+    return [mem[off[i]:off[i + 1]] for i in range(len(off) - 1)], in_component.cpu().numpy().astype(np.uint32)
+
+
+def compute_partition(args, embeddings, edg_source, edg_target, diff, xyz=0, seed=0):
+    """(pred_components, pred_in_component) on the device — ref: losses.py:67-89.  Edge weights from
+    ops.lp_edge_weight (cast to float32), ver_value = [embeddings | spatial_emb * xyz], lambda = reg_strength /
+    (4 k_nn_adj), cutoff = CP_cutoff, weight_decay = 0.7.  Feed the result to
+    spg_partition.compute_weight_loss(..., partition=...)."""
+    dev = _device(embeddings, diff)
+    d = diff if torch.is_tensor(diff) else torch.as_tensor(np.asarray(diff))
+    edge_weight = ops.lp_edge_weight(d.detach().to(device=dev, dtype=torch.float32),
+                                     args.edge_weight_threshold).to(torch.float32)
+    ver_value = embeddings.detach().to(device=dev, dtype=torch.float32)
+    use_spatial = 0
+    if args.spatial_emb > 0:
+        x = xyz if torch.is_tensor(xyz) else torch.as_tensor(np.asarray(xyz))
+        ver_value = torch.cat([ver_value, (args.spatial_emb * x.to(device=dev, dtype=torch.float32))], 1)
+        use_spatial = 1
+    return cutpursuit(ver_value.contiguous(), edg_source, edg_target, edge_weight,
+                      args.reg_strength / (4 * args.k_nn_adj), cutoff=args.CP_cutoff, spatial=use_spatial,
+                      weight_decay=0.7, seed=seed)
