@@ -878,6 +878,40 @@ int spg_cp_energy(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t 
 int spg_cp_output(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
                   int64_t* in_component, int64_t* offsets, int64_t* members, spg_stream_t stream);
 
+/* ---------------------------------------------------------------- Delaunay triangulation
+ * The exact 3D Delaunay triangulation of a float32 cloud (the one compute_sp_graph takes as simplices; ref:
+ * partition/graphs.py:82, scipy.spatial.Delaunay), one stage per call; spg_delaunay.py runs the rounds.  n points
+ * (< 2^31 - 1), a store of cap tetrahedra (8 <= cap <= 2^29).  One workspace of spg_dt_workspace(n, cap) bytes
+ * (256-byte aligned) holds the whole state; every call takes the same (n, cap, workspace).
+ *
+ * spg_dt_setup: out[0] (host) = status (1: a non-finite coordinate), out[1] = the unique points (exact duplicates,
+ *   -0 equal to +0, keep their smallest index); the points ranked lexicographically and ordered by a Morton key.
+ * spg_dt_init: out[0] = status (2: fewer than 4 affinely independent points, 4: a walk did not end); the first
+ *   tetrahedron, its four infinite neighbours, every point located.
+ * spg_dt_cavities (big_point -1, or the one nominee whose cavity outgrew its buffer): nominate, grow the cavities,
+ *   claim, check; out[0..7] (host) = nominees, winners, new tetrahedra, overflowing nominees, the smallest of
+ *   them, free slots, store top, largest cavity so far.
+ * spg_dt_commit: out[0] (host) = 1 when the winners need more slots than the store holds (nothing is written);
+ *   else the winners' cavities are retriangulated, the displaced points relocated, out[1] = status (4: a walk did
+ *   not end, 8: a cavity that is not a ball).
+ * spg_dt_grow: copies the state into a workspace of spg_dt_workspace(n, new_cap) bytes.
+ * spg_dt_output: with simplices NULL, count (host) = the finite tetrahedra; else simplices [count, 4] (device,
+ *   int32) = them in input ids, each rotated by an even permutation to (smallest, second smallest, ...), rows
+ *   sorted.  The adjacency is consumed: output is the last call on a workspace.                            */
+int spg_dt_workspace(int64_t n, int64_t cap, int64_t* bytes);
+int spg_dt_setup(const float* xyz, int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t* out,
+                 spg_stream_t stream);
+int spg_dt_init(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t* out,
+                spg_stream_t stream);
+int spg_dt_cavities(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t big_point,
+                    int64_t* out, spg_stream_t stream);
+int spg_dt_commit(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t* out,
+                  spg_stream_t stream);
+int spg_dt_grow(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t new_cap,
+                void* new_workspace, int64_t new_workspace_bytes, spg_stream_t stream);
+int spg_dt_output(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t* count, int* simplices,
+                  spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

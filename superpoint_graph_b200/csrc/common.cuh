@@ -104,6 +104,14 @@ enum KernelId {
     K_CP_SPLIT,
     K_CP_MERGE,
     K_CP_ENERGY,
+    K_DT_SETUP,
+    K_DT_INIT,
+    K_DT_NOMINATE,
+    K_DT_GROW,
+    K_DT_CHECK,
+    K_DT_COMMIT,
+    K_DT_RELOCATE,
+    K_DT_OUTPUT,
     K_COUNT
 };
 

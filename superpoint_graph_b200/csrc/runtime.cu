@@ -37,6 +37,8 @@ static const char* kKernelNames[K_COUNT] = {
     "cp_graph",          "cp_members",         "cp_kmeans",           "cp_centers",
     "cp_capacities",     "cp_maxflow",         "cp_colour",           "cp_activate",
     "cp_split",          "cp_merge",           "cp_energy",
+    "dt_setup",          "dt_init",            "dt_nominate",         "dt_grow",
+    "dt_check",          "dt_commit",          "dt_relocate",         "dt_output",
 };
 
 struct Record {

@@ -1581,3 +1581,56 @@ def prune_reduce(xyz, rgb, labels, n_labels, objects, n_objects, chunk_rows, ws,
               int(chunk_rows), ws, ws.numel(), int(m), xyz_out, rgb_out, labels_out, objects_out,
               _lib.current_stream())
     return xyz_out, rgb_out, labels_out, objects_out
+
+
+# ------------------------------------------------------------- Delaunay triangulation (csrc/delaunay.cu)
+class DelaunayStore(object):
+    """The workspace of one device triangulation: n points, a store of `cap` tetrahedra; see spg_dt_*."""
+
+    def __init__(self, n, cap, device):
+        self.n, self.cap, self.device = int(n), int(cap), device
+        self.ws = _workspace("spg_dt_workspace", device, self.n, self.cap)
+        self.out = torch.zeros(8, dtype=torch.int64)
+
+    def _call(self, name, *args):
+        _lib.call(name, self.n, self.cap, self.ws, self.ws.numel(), *args, _lib.current_stream())
+
+    def setup(self, xyz):
+        """(status, unique points); status 1: a non-finite coordinate."""
+        _need_cuda(xyz)
+        assert xyz.dtype == torch.float32 and xyz.is_contiguous() and xyz.shape == (self.n, 3)
+        _lib.call("spg_dt_setup", xyz, self.n, self.cap, self.ws, self.ws.numel(), self.out, _lib.current_stream())
+        return int(self.out[0]), int(self.out[1])
+
+    def init(self):
+        """status: 2 fewer than 4 affinely independent points, 4 a walk that did not end."""
+        self._call("spg_dt_init", self.out)
+        return int(self.out[0])
+
+    def cavities(self, big_point=-1):
+        """(nominees, winners, new tetrahedra, overflowing nominees, smallest overflowing, free slots, top,
+        largest cavity)."""
+        self._call("spg_dt_cavities", int(big_point), self.out)
+        return tuple(int(v) for v in self.out)
+
+    def commit(self):
+        """(short of slots, status): nothing is written when the store is short."""
+        self._call("spg_dt_commit", self.out)
+        return int(self.out[0]), int(self.out[1])
+
+    def grow(self, cap):
+        """Moves the state into a workspace for `cap` tetrahedra."""
+        nbytes = torch.zeros(1, dtype=torch.int64)
+        _lib.call("spg_dt_workspace", self.n, int(cap), nbytes)
+        ws = torch.empty(int(nbytes[0]), dtype=torch.uint8, device=self.device)
+        self._call("spg_dt_grow", int(cap), ws, ws.numel())
+        self.ws, self.cap = ws, int(cap)
+
+    def output(self):
+        """int32 [T, 4] on the device: the finite tetrahedra, canonical (consumes the adjacency)."""
+        count = torch.zeros(1, dtype=torch.int64)
+        self._call("spg_dt_output", count, None)
+        simplices = torch.empty((int(count[0]), 4), dtype=torch.int32, device=self.device)
+        if simplices.shape[0]:
+            self._call("spg_dt_output", count, simplices)
+        return simplices
