@@ -912,6 +912,63 @@ int spg_dt_grow(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes
 int spg_dt_output(int64_t n, int64_t cap, void* workspace, int64_t workspace_bytes, int64_t* count, int* simplices,
                   spg_stream_t stream);
 
+/* ---------------------------------------------------------------- learned partition's graph structure
+ * The structure graph_processing.py builds before write_structure (ref: supervized_partition/graph_processing.py:
+ * 144-193), on the device.  status words (device, uint32) are zeroed by the call that fills them; 2: an id outside
+ * [0, n).
+ *
+ * spg_st_vor_count: the Voronoi candidates of compute_graph_nn_2(voronoi > 0) (ref: partition/graphs.py:44-49):
+ *   candidate c = p n_tets + r is (simplices[r][a_p], simplices[r][b_p]) for the column pairs (a_p, b_p) = (0,1),
+ *   (0,2), (0,3), (1,2), (1,3), (2,3) (simplices [n_tets, 4], int64 when ids64 else int32, n_tets <= 2^29); it is
+ *   kept when d2 = (dx dx + dy dy) + dz dz, rounded op by op in float32, is < voronoi (the float32 of the caller's
+ *   threshold).  block_counts [spg_st_vor_blocks(n_tets) + 1] (device, int64) = the kept candidates of every chunk,
+ *   and their total in the last entry.
+ * spg_st_vor_build (workspace: spg_st_vor_workspace(n, n_tets, n k_nn1, n_kept) bytes, 256-byte aligned; n_kept
+ *   read back from the count): distances [n_kept] = d2 of the kept candidates in candidate order (graphs.py:64);
+ *   source, target [n_kept + n k_nn1] (device, int64) = the union of the kept candidates and the k-NN edges
+ *   (i, knn_target[i k_nn1 + j]) deduplicated and sorted by (target, source) (np.unique of source + n target,
+ *   graphs.py:53-62); n_edges [1] (device, int64) = the number of edges written.
+ * spg_st_cc (workspace: spg_st_cc_workspace(n_ver) bytes): libply_c's connected_comp with cutoff 0 (ref:
+ *   partition/ply_c/connected_components.cpp:17-40): the components of the edges whose active byte, read as a
+ *   signed char, is > 0; in_component [n_ver] numbered by smallest vertex (boost's numbering), offsets
+ *   [n_ver + 1] (first n_comp + 1 used) and members [n_ver] (ascending within a component), n_comp [1] (device,
+ *   all int64).
+ * spg_st_argmax: out [n] (int64) = add + the first column of maximum value of a[i, col0:cols) (np.argmax);
+ *   zero_empty: 0 where a[i, col0:] sums to 0; weight [n] (float32, may be NULL) = 0 there, else 1
+ *   (graph_processing.py:126,152-154,161-162,168).
+ * spg_st_transitions: is_transition [n_edges] (uint8) = lab[s] != lab[t] (mode 0; :149,165,169),
+ *   hs != ht * (hs != 0) * (ht != 0) (mode 1, numpy's precedence of :155-156) or lab[s] == lab[t] (mode 2).
+ * spg_st_select (workspace: spg_st_select_workspace(n) bytes): index = the ascending i with (flags[i] != 0) ==
+ *   want, count [1] (device, int64) = their number.
+ * spg_st_gather_rows: out[j] = the row_bytes bytes of row index[j] of src [n_rows].
+ * spg_st_points: with bounds = spg_knn_bounds' words of xyz: elevation [n] = z - min z in float32 (plane 0,
+ *   :186) or float32(z - (x c0 + y c1 + b)) in fp64 (plane 1, :184); xyn [n, 2] = (xy - min) / (max - min +
+ *   1e-8f) in float32 (:189-190); low [n] (uint8) = z - min z < 0.5f (:182); geof [n, 4]: column 3 doubled in
+ *   place (:177).  Every output may be NULL.                                                               */
+int64_t spg_st_vor_blocks(int64_t n_tets);
+int spg_st_vor_workspace(int64_t n, int64_t n_tets, int64_t n_knn, int64_t n_kept, int64_t* bytes);
+int spg_st_vor_count(const float* xyz, int64_t n, const void* simplices, int ids64, int64_t n_tets, float voronoi,
+                     int64_t* block_counts, uint32_t* status, spg_stream_t stream);
+int spg_st_vor_build(const float* xyz, int64_t n, const void* simplices, int ids64, int64_t n_tets, float voronoi,
+                     const int64_t* block_counts, const int64_t* knn_target, int64_t k_nn1, int64_t n_kept,
+                     void* workspace, int64_t workspace_bytes, float* distances, int64_t* source, int64_t* target,
+                     int64_t* n_edges, uint32_t* status, spg_stream_t stream);
+int spg_st_cc_workspace(int64_t n_ver, int64_t* bytes);
+int spg_st_cc(const int64_t* src, const int64_t* tgt, const uint8_t* active, int64_t n_ver, int64_t n_edges,
+              void* workspace, int64_t workspace_bytes, int64_t* in_component, int64_t* offsets, int64_t* members,
+              int64_t* n_comp, uint32_t* status, spg_stream_t stream);
+int spg_st_argmax(const int64_t* a, int64_t n, int64_t cols, int64_t col0, int64_t add, int zero_empty,
+                  int64_t* out, float* weight, spg_stream_t stream);
+int spg_st_transitions(const int64_t* lab, int64_t n, const int64_t* src, const int64_t* tgt, int64_t n_edges,
+                       int mode, uint8_t* is_transition, uint32_t* status, spg_stream_t stream);
+int spg_st_select_workspace(int64_t n, int64_t* bytes);
+int spg_st_select(const uint8_t* flags, int64_t n, int want, void* workspace, int64_t workspace_bytes, int64_t* index,
+                  int64_t* count, spg_stream_t stream);
+int spg_st_gather_rows(const void* src, int64_t n_rows, int64_t row_bytes, const int64_t* index, int64_t m, void* out,
+                       uint32_t* status, spg_stream_t stream);
+int spg_st_points(const float* xyz, int64_t n, const uint32_t* bounds, int plane, double c0, double c1, double b,
+                  float* elevation, float* xyn, uint8_t* low, float* geof, spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

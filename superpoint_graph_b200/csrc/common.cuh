@@ -112,6 +112,11 @@ enum KernelId {
     K_DT_COMMIT,
     K_DT_RELOCATE,
     K_DT_OUTPUT,
+    K_ST_VOR,
+    K_ST_CC,
+    K_ST_LABELS,
+    K_ST_SELECT,
+    K_ST_POINTS,
     K_COUNT
 };
 

@@ -6,9 +6,8 @@
 //   lp_dist_bwd    dL/dembeddings, a thread per (vertex, column) over the vertex's incidences in a fixed order
 //   lp_loss_fwd    compute_loss: fp64 per-block partials over a fixed grid, merged in a fixed order
 //   lp_loss_bwd    dL/ddiff
-//   lp_cc          connected components of the edges with is_transition + pred_transition == 0 (union-find,
-//                  parents only ever point to smaller vertices, so every root is its component's smallest vertex
-//                  and components are numbered by it: libply_c's connected_comp with cutoff 0)
+//   lp_cc          connected components of the edges with is_transition + pred_transition == 0 (the union-find
+//                  of cc.cuh: libply_c's connected_comp with cutoff 0)
 //   lp_xpart       crosspartition weights: a radix sort of the transition edges' unordered component pairs,
 //                  run lengths by binary search in the sorted keys
 //   lp_seal        SEAL weights: a radix sort of (component, object) pairs, run lengths, per-component maximum
@@ -23,6 +22,7 @@
 
 #include <cub/cub.cuh>
 
+#include "cc.cuh"
 #include "workspace.cuh"
 
 namespace spg {
@@ -240,20 +240,6 @@ lp_loss_bwd_kernel(const float* __restrict__ diff, const float* __restrict__ w, 
 }
 
 // ------------------------------------------------------------------------------------------ connected components
-__device__ __forceinline__ int cc_find(int* p, int x) {
-    volatile int* vp = p;
-    int cur = vp[x];
-    if (cur != x) {
-        int prev = x, next;
-        while (cur > (next = vp[cur])) {  // path halving; parents point to smaller vertices, roots to themselves
-            vp[prev] = next;
-            prev = cur;
-            cur = next;
-        }
-    }
-    return cur;
-}
-
 __global__ void __launch_bounds__(LP_THREADS)
 lp_cc_init_kernel(const int64_t* __restrict__ src, const int64_t* __restrict__ tgt, const uint8_t* __restrict__ is_trans,
                   const int64_t* __restrict__ pic, int64_t n_ver, int64_t n_edges, int* __restrict__ parent,
@@ -276,38 +262,7 @@ lp_cc_hook_kernel(const int64_t* __restrict__ src, const int64_t* __restrict__ t
     if (e >= n_edges || is_trans[e] != 0) return;
     const int64_t s = src[e], t = tgt[e];
     if (!in_range(s, n_ver) || !in_range(t, n_ver) || pic[s] != pic[t]) return;
-    int ru = cc_find(parent, (int)s), rv = cc_find(parent, (int)t);
-    while (ru != rv) {
-        const int hi = ru > rv ? ru : rv, lo = ru > rv ? rv : ru;
-        if (atomicCAS(parent + hi, hi, lo) == hi) break;
-        ru = cc_find(parent, ru);
-        rv = cc_find(parent, rv);
-    }
-}
-
-__global__ void __launch_bounds__(LP_THREADS)
-lp_cc_flatten_kernel(int* __restrict__ parent, int64_t n_ver, int* __restrict__ is_root) {
-    SPG_PDL_ENTRY();
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= n_ver) return;
-    const int r = cc_find(parent, (int)v);
-    parent[v] = r;
-    is_root[v] = r == (int)v;
-}
-
-// components numbered by their smallest vertex; sizes by integer atomics
-__global__ void __launch_bounds__(LP_THREADS)
-lp_cc_label_kernel(const int* __restrict__ parent, const int* __restrict__ root_rank, const int* __restrict__ is_root,
-                   int64_t n_ver, int* __restrict__ in_comp, int* __restrict__ comp_size, int* __restrict__ n_comp) {
-    SPG_PDL_ENTRY();
-    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= n_ver) return;
-    int r = parent[v];
-    while (parent[r] != r) r = parent[r];
-    const int c = root_rank[r];
-    in_comp[v] = c;
-    atomicAdd(comp_size + c, 1);
-    if (v == n_ver - 1) *n_comp = root_rank[v] + is_root[v];
+    cc_union(parent, (int)s, (int)t);
 }
 
 // ------------------------------------------------------------------------------------------ crosspartition
@@ -696,9 +651,9 @@ int spg_lp_xpart(const int64_t* src, const int64_t* tgt, const uint8_t* is_trans
     if (n_edges > 0)
         SPG_LAUNCH(K_LP_CC, s, lp_cc_hook_kernel, grid_of(n_edges), LP_THREADS, 0, src, tgt, is_transition,
                    pred_in_component, n_ver, n_edges, w.parent);
-    SPG_LAUNCH(K_LP_CC, s, lp_cc_flatten_kernel, grid_of(n_ver), LP_THREADS, 0, w.parent, n_ver, w.is_root);
+    SPG_LAUNCH(K_LP_CC, s, cc_flatten_kernel, grid_of(n_ver), CC_THREADS, 0, w.parent, n_ver, w.is_root);
     SPG_CUB(w.cub, cub::DeviceScan::ExclusiveSum, (const int*)w.is_root, w.root_rank, (int)n_ver, s);
-    SPG_LAUNCH(K_LP_CC, s, lp_cc_label_kernel, grid_of(n_ver), LP_THREADS, 0, (const int*)w.parent,
+    SPG_LAUNCH(K_LP_CC, s, cc_label_kernel<int>, grid_of(n_ver), CC_THREADS, 0, (const int*)w.parent,
                (const int*)w.root_rank, (const int*)w.is_root, n_ver, (int*)in_component_x, (int*)comp_size,
                (int*)n_comp);
     if (n_edges == 0) return launch_status();

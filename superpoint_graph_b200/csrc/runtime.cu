@@ -39,6 +39,8 @@ static const char* kKernelNames[K_COUNT] = {
     "cp_split",          "cp_merge",           "cp_energy",
     "dt_setup",          "dt_init",            "dt_nominate",         "dt_grow",
     "dt_check",          "dt_commit",          "dt_relocate",         "dt_output",
+    "st_vor",            "st_cc",              "st_labels",           "st_select",
+    "st_points",
 };
 
 struct Record {

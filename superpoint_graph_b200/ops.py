@@ -1634,3 +1634,117 @@ class DelaunayStore(object):
         if simplices.shape[0]:
             self._call("spg_dt_output", count, simplices)
         return simplices
+
+
+# ------------------------------------------------------------- learned partition's structure (csrc/structure.cu)
+def _status(dev):
+    return torch.empty(1, dtype=torch.int32, device=dev)
+
+
+def st_vor_count(xyz, simplices, voronoi):
+    """(block_counts int64 [blocks + 1], status int32 [1]; 2: an id outside [0, n)) on the device;
+    block_counts[-1] is the number of kept candidates.  voronoi: the float32 threshold.  See spg_st_vor_count."""
+    _need_cuda(xyz, simplices)
+    assert simplices.dtype in (torch.int32, torch.int64) and simplices.is_contiguous()
+    dev, t = xyz.device, simplices.shape[0]
+    counts = torch.empty(int(_lib.lib().spg_st_vor_blocks(int(t))) + 1, dtype=torch.int64, device=dev)
+    status = _status(dev)
+    _lib.call("spg_st_vor_count", xyz, xyz.shape[0], simplices, int(simplices.dtype == torch.int64), int(t),
+              float(voronoi), counts, status, _lib.current_stream())
+    return counts, status
+
+
+def st_vor_build(xyz, simplices, voronoi, counts, knn_target, k1, n_kept):
+    """(distances float32 [n_kept], source, target int64 [n_kept + n k1], n_edges int64 [1], status int32 [1]) on
+    the device: the first n_edges of source / target are the deduplicated union.  See spg_st_vor_build."""
+    _need_cuda(xyz, simplices, counts, knn_target)
+    assert knn_target.dtype == torch.int64 and knn_target.is_contiguous()
+    dev, n, t = xyz.device, xyz.shape[0], simplices.shape[0]
+    ws = _workspace("spg_st_vor_workspace", dev, n, t, n * k1, n_kept)
+    distances = torch.empty(n_kept, dtype=torch.float32, device=dev)
+    source = torch.empty(n_kept + n * k1, dtype=torch.int64, device=dev)
+    target = torch.empty(n_kept + n * k1, dtype=torch.int64, device=dev)
+    n_edges = torch.empty(1, dtype=torch.int64, device=dev)
+    status = _status(dev)
+    _lib.call("spg_st_vor_build", xyz, n, simplices, int(simplices.dtype == torch.int64), int(t), float(voronoi),
+              counts, knn_target, int(k1), int(n_kept), ws, ws.numel(), distances, source, target, n_edges, status,
+              _lib.current_stream())
+    return distances, source, target, n_edges, status
+
+
+def st_cc(src, tgt, active, n_ver):
+    """(in_component, offsets [n_ver + 1], members, n_comp [1], all int64, status int32 [1]) on the device; see
+    spg_st_cc.  active: uint8 [E], an edge is active where the byte read as a signed char is > 0."""
+    _need_cuda(src, tgt, active)
+    assert src.dtype == tgt.dtype == torch.int64 and active.dtype == torch.uint8
+    dev = src.device
+    ws = _workspace("spg_st_cc_workspace", dev, n_ver)
+    in_comp = torch.empty(n_ver, dtype=torch.int64, device=dev)
+    offsets = torch.empty(n_ver + 1, dtype=torch.int64, device=dev)
+    members = torch.empty(n_ver, dtype=torch.int64, device=dev)
+    n_comp = torch.empty(1, dtype=torch.int64, device=dev)
+    status = _status(dev)
+    _lib.call("spg_st_cc", src, tgt, active, int(n_ver), src.shape[0], ws, ws.numel(), in_comp, offsets, members,
+              n_comp, status, _lib.current_stream())
+    return in_comp, offsets, members, n_comp, status
+
+
+def st_argmax(a, col0, add, zero_empty=False, want_weight=False):
+    """(out int64 [n], weight float32 [n] or None): add + the first argmax of a[:, col0:]; see spg_st_argmax."""
+    _need_cuda(a)
+    assert a.dtype == torch.int64 and a.dim() == 2 and a.is_contiguous()
+    n, cols = a.shape
+    out = torch.empty(n, dtype=torch.int64, device=a.device)
+    weight = torch.empty(n, dtype=torch.float32, device=a.device) if want_weight else None
+    _lib.call("spg_st_argmax", a, int(n), int(cols), int(col0), int(add), int(bool(zero_empty)), out, weight,
+              _lib.current_stream())
+    return out, weight
+
+
+ST_DIFFERENT, ST_INPAINT, ST_EQUAL = 0, 1, 2
+
+
+def st_transitions(lab, src, tgt, mode):
+    """(uint8 [E], status int32 [1]; 2: an id outside [0, n)): mode ST_DIFFERENT lab[s] != lab[t], ST_INPAINT
+    graph_processing.py:155-156, ST_EQUAL lab[s] == lab[t]; see spg_st_transitions."""
+    _need_cuda(lab, src, tgt)
+    assert lab.dtype == src.dtype == tgt.dtype == torch.int64
+    out = torch.empty(src.shape[0], dtype=torch.uint8, device=src.device)
+    status = _status(src.device)
+    _lib.call("spg_st_transitions", lab, lab.shape[0], src, tgt, src.shape[0], int(mode), out, status,
+              _lib.current_stream())
+    return out, status
+
+
+def st_select(flags, want):
+    """(index int64 [n], count int64 [1]) on the device: the first count entries of index are the ascending i with
+    (flags[i] != 0) == want; see spg_st_select."""
+    _need_cuda(flags)
+    assert flags.dtype == torch.uint8 and flags.is_contiguous()
+    dev, n = flags.device, flags.shape[0]
+    ws = _workspace("spg_st_select_workspace", dev, n)
+    index = torch.empty(n, dtype=torch.int64, device=dev)
+    count = torch.empty(1, dtype=torch.int64, device=dev)
+    _lib.call("spg_st_select", flags, int(n), int(bool(want)), ws, ws.numel(), index, count, _lib.current_stream())
+    return index, count
+
+
+def st_gather_rows(src, index, m):
+    """(src[index[:m]], status int32 [1]) on the device: whole rows of a contiguous tensor."""
+    _need_cuda(src, index)
+    assert src.is_contiguous() and index.dtype == torch.int64
+    out = torch.empty((m,) + tuple(src.shape[1:]), dtype=src.dtype, device=src.device)
+    status = _status(src.device)
+    row_bytes = src[0].numel() * src.element_size() if src.shape[0] else 1
+    _lib.call("spg_st_gather_rows", src, src.shape[0], int(row_bytes), index, int(m), out, status,
+              _lib.current_stream())
+    return out, status
+
+
+def st_points(xyz, bounds, plane=None, elevation=None, xyn=None, low=None, geof=None):
+    """Fills the given outputs (elevation float32 [n], xyn float32 [n, 2], low uint8 [n], geof float32 [n, 4]:
+    column 3 doubled in place); plane = (c0, c1, b) or None.  bounds: knn_bounds(xyz).  See spg_st_points."""
+    _need_cuda(xyz, bounds)
+    c0, c1, b = (0.0, 0.0, 0.0) if plane is None else plane
+    _lib.call("spg_st_points", xyz, xyz.shape[0], bounds, int(plane is not None), float(c0), float(c1), float(b),
+              elevation, xyn, low, geof, _lib.current_stream())

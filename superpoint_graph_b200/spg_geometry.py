@@ -159,11 +159,11 @@ def compute_graph_nn(xyz, k_nn):
 def compute_graph_nn_2(xyz, k_nn1, k_nn2, voronoi=0.0):
     """The k_nn1 graph and the k_nn2 neighbour list from one query (ref: partition/graphs.py:26-70):
     (graph, target2) with graph as compute_graph_nn's for the first k_nn1 neighbours and target2 int64 [n k_nn2].
-    The Delaunay edges of voronoi > 0 are not computed here."""
+    The Delaunay edges of voronoi > 0 are spg_structure.compute_graph_nn_2's."""
     assert k_nn1 <= k_nn2, "knn1 must be smaller than knn2"
     if voronoi > 0:
-        raise NotImplementedError("voronoi > 0 (Delaunay edges) is not computed on the device; use the reference's "
-                                  "partition/graphs.py:compute_graph_nn_2")
+        raise NotImplementedError("voronoi > 0 (Delaunay edges) is not computed here; use "
+                                  "spg_structure.compute_graph_nn_2")
     n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
     k_nn1 = _check_k(k_nn1, n, "k_nn1")
     k_nn2 = _check_k(k_nn2, n, "k_nn2")
