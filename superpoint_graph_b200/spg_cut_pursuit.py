@@ -20,6 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
+from ._inputs import check_dtype, check_ints, device_of, on_device
 
 __all__ = ["Components", "cutpursuit", "to_numpy", "compute_partition"]
 
@@ -61,35 +62,6 @@ def unary_weights(weight_decay):
         u = np.float32(u * wd)
         out.append(float(u))
     return out
-
-
-def _device(*xs):
-    for x in xs:
-        if torch.is_tensor(x) and x.is_cuda:
-            return x.device
-    return torch.device("cuda", torch.cuda.current_device())
-
-
-def _float32(a, name, dev):
-    if torch.is_tensor(a):
-        if a.dtype != torch.float32:
-            raise TypeError("%s must be float32 (got %s)" % (name, a.dtype))
-        return a.detach().to(dev).contiguous()
-    a = np.asarray(a)
-    if a.dtype != np.float32:
-        raise TypeError("%s must be float32 (got %s)" % (name, a.dtype))
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-
-def _ids(a, name, dev):
-    if torch.is_tensor(a):
-        if a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
-            raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
-        return a.detach().to(device=dev, dtype=torch.int64).reshape(-1).contiguous()
-    a = np.asarray(a)
-    if a.dtype.kind not in "iu":
-        raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
-    return torch.from_numpy(np.ascontiguousarray(a.reshape(-1), dtype=np.int64)).to(dev)
 
 
 class State:
@@ -233,25 +205,19 @@ def prepare(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial=0,
         raise ValueError("weight_decay must be > 0 (got %r)" % (weight_decay,))
     if not math.isfinite(float(reg_strength)):
         raise ValueError("reg_strength must be finite (got %r)" % (reg_strength,))
-    for a, name in ((obs, "obs"), (edge_weight, "edge_weight")):
-        dt = a.dtype if torch.is_tensor(a) else np.asarray(a).dtype
-        if dt not in (torch.float32, np.float32):
-            raise TypeError("%s must be float32 (got %s)" % (name, dt))
-    for a, name in ((source, "source"), (target, "target")):
-        if torch.is_tensor(a):
-            if a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
-                raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
-        elif np.asarray(a).dtype.kind not in "iu":
-            raise TypeError("%s must hold integers (got %s)" % (name, np.asarray(a).dtype))
+    check_dtype(obs, "obs", "float32")
+    check_dtype(edge_weight, "edge_weight", "float32")
+    check_ints(source, "source")
+    check_ints(target, "target")
     sizes = [a.numel() if torch.is_tensor(a) else np.asarray(a).size for a in (source, target, edge_weight)]
     if len(set(sizes)) != 1:
         raise ValueError("source, target and edge_weight must have one entry per edge (got %d, %d, %d)"
                          % tuple(sizes))
-    dev = _device(obs, source, target, edge_weight)
-    obs_t = _float32(obs, "obs", dev)
-    w = _float32(edge_weight, "edge_weight", dev).reshape(-1)
-    src = _ids(source, "source", dev)
-    tgt = _ids(target, "target", dev)
+    dev = device_of(obs, source, target, edge_weight)
+    obs_t = on_device(obs, dev)
+    w = on_device(edge_weight, dev).reshape(-1)
+    src = on_device(source, dev, int64=True).reshape(-1)
+    tgt = on_device(target, dev, int64=True).reshape(-1)
     with torch.cuda.device(dev):
         state = State(obs_t, src, tgt, w)
     if state.status & 4:
@@ -289,7 +255,7 @@ def compute_partition(args, embeddings, edg_source, edg_target, diff, xyz=0, see
     ops.lp_edge_weight (cast to float32), ver_value = [embeddings | spatial_emb * xyz], lambda = reg_strength /
     (4 k_nn_adj), cutoff = CP_cutoff, weight_decay = 0.7.  Feed the result to
     spg_partition.compute_weight_loss(..., partition=...)."""
-    dev = _device(embeddings, diff)
+    dev = device_of(embeddings, diff)
     d = diff if torch.is_tensor(diff) else torch.as_tensor(np.asarray(diff))
     edge_weight = ops.lp_edge_weight(d.detach().to(device=dev, dtype=torch.float32),
                                      args.edge_weight_threshold).to(torch.float32)

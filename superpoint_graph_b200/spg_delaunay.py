@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .spg_geometry import _device_of, _n_rows, _xyz
+from ._inputs import check_dtype, device_of, n_points, on_device
 
 __all__ = ["delaunay", "to_numpy", "last_stats"]
 
@@ -40,25 +40,17 @@ def delaunay(xyz, capacity=None):
     ValueError: a non-finite coordinate, fewer than 4 affinely independent unique points, n >= 2^31 - 1, a shape
     other than [n, 3], a triangulation of more than 2^29 tetrahedra (the store's limit; about 7.7 10^7 points in
     general position), a capacity outside [8, 2^29].  TypeError: xyz not float32.  capacity: the initial store of tetrahedra (it grows as needed)."""
+    n = n_points(check_dtype(xyz, "xyz", "float32"))
     if torch.is_tensor(xyz):
-        if xyz.dtype != torch.float32:
-            raise TypeError("xyz must be float32 (got %s)" % xyz.dtype)
-        n = _n_rows(tuple(xyz.shape))
-        if not xyz.is_cuda:
-            ops._need_cuda(xyz)
-    else:
-        a = np.asarray(xyz)
-        if a.dtype != np.float32:
-            raise TypeError("xyz must be float32 (got %s)" % a.dtype)
-        n = _n_rows(a.shape)
+        ops._need_cuda(xyz)
     if n < 4:
         raise ValueError("fewer than 4 affinely independent points (%d points)" % n)
     cap = int(capacity) if capacity is not None else _initial_cap(n)
     if not 8 <= cap <= _MAX_CAP:
         raise ValueError("capacity must be in [8, 2^29] (got %d)" % cap)
-    dev = _device_of(xyz)
+    dev = device_of(xyz)
     with torch.cuda.device(dev):
-        x = _xyz(xyz, dev)
+        x = on_device(xyz, dev)
         store = ops.DelaunayStore(n, cap, dev)
         status, unique = store.setup(x)
         if status & 1:

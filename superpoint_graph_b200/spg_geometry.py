@@ -25,46 +25,11 @@ import numpy as np
 import torch
 
 from . import ops
+from ._inputs import check_dtype, check_ints, device_of, n_points, on_device
 
 __all__ = ["compute_graph_nn", "compute_graph_nn_2", "compute_geof"]
 
-_MAX_N = 2 ** 31 - 1
 _GRID_DIM = 2 ** 21 - 1  # cells per axis (21 bits of the 63-bit cell key)
-
-
-def _device_of(*arrays):
-    for a in arrays:
-        if torch.is_tensor(a) and a.is_cuda:
-            return a.device
-    return torch.device("cuda", torch.cuda.current_device())
-
-
-def _n_rows(shape):
-    if len(shape) != 2 or shape[1] != 3:
-        raise ValueError("xyz must be [n, 3] (got shape %s)" % (tuple(shape),))
-    if shape[0] >= _MAX_N:
-        raise ValueError("%d points; clouds of 2^31 - 1 points or more are not supported" % shape[0])
-    return int(shape[0])
-
-
-def _dtype(xyz):
-    dt = xyz.dtype if torch.is_tensor(xyz) else np.asarray(xyz).dtype
-    if dt != (torch.float32 if torch.is_tensor(xyz) else np.float32):
-        raise TypeError("xyz must be float32 (got %s)" % dt)
-
-
-def _xyz(xyz, device):
-    """float32 [n, 3] contiguous on the device; other dtypes are refused, never rounded."""
-    if torch.is_tensor(xyz):
-        if xyz.dtype != torch.float32:
-            raise TypeError("xyz must be float32 (got %s)" % xyz.dtype)
-        _n_rows(xyz.shape)
-        return xyz.to(device).contiguous()
-    a = np.asarray(xyz)
-    if a.dtype != np.float32:
-        raise TypeError("xyz must be float32 (got %s)" % a.dtype)
-    _n_rows(a.shape)
-    return torch.from_numpy(np.ascontiguousarray(a)).to(device)
 
 
 def _check_k(k, n, what):
@@ -146,11 +111,11 @@ def _knn(xyz, k, k1, want_target2):
 def compute_graph_nn(xyz, k_nn):
     """The k-NN graph (ref: partition/graphs.py:11-24): dict is_nn=True, source = repeat(arange(n), k_nn),
     target (int64 [n k_nn], row-major) and distances (float32 [n k_nn])."""
-    n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
+    n = n_points(np.shape(xyz))
     k_nn = _check_k(k_nn, n, "k_nn")
-    _dtype(xyz)
-    dev = _device_of(xyz)
-    xyz = _xyz(xyz, dev)
+    check_dtype(xyz, "xyz", "float32")
+    dev = device_of(xyz)
+    xyz = on_device(xyz, dev)
     with torch.cuda.device(dev):
         source, target, distances, _ = _knn(xyz, k_nn, k_nn, False)
     return {"is_nn": True, "source": source, "target": target, "distances": distances}
@@ -164,12 +129,12 @@ def compute_graph_nn_2(xyz, k_nn1, k_nn2, voronoi=0.0):
     if voronoi > 0:
         raise NotImplementedError("voronoi > 0 (Delaunay edges) is not computed here; use "
                                   "spg_structure.compute_graph_nn_2")
-    n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
+    n = n_points(np.shape(xyz))
     k_nn1 = _check_k(k_nn1, n, "k_nn1")
     k_nn2 = _check_k(k_nn2, n, "k_nn2")
-    _dtype(xyz)
-    dev = _device_of(xyz)
-    xyz = _xyz(xyz, dev)
+    check_dtype(xyz, "xyz", "float32")
+    dev = device_of(xyz)
+    xyz = on_device(xyz, dev)
     with torch.cuda.device(dev):
         source, target, distances, target2 = _knn(xyz, k_nn2, k_nn1, True)
     return {"is_nn": True, "source": source, "target": target, "distances": distances}, target2
@@ -179,26 +144,18 @@ def compute_geof(xyz, target, k_nn):
     """Linearity, planarity, scattering and verticality of every vertex and its k_nn neighbours
     target[k_nn i : k_nn i + k_nn] (ref: partition/ply_c/ply_c.cpp:384-462), float32 [n, 4], unscaled (the callers
     double column 3).  IndexError for an id outside [0, n) (one read-back), ValueError for a short target."""
-    n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
+    n = n_points(np.shape(xyz))
     if isinstance(k_nn, bool) or int(k_nn) != k_nn or k_nn < 1:
         raise ValueError("k_nn must be a positive integer (got %r)" % (k_nn,))
     k_nn = int(k_nn)
-    if torch.is_tensor(target):
-        if target.dtype.is_floating_point or target.dtype == torch.bool:
-            raise TypeError("target must hold integer ids (got %s)" % target.dtype)
-        t = target.reshape(-1)
-    else:
-        t = np.asarray(target).reshape(-1)
-        if t.dtype.kind not in "iu":
-            raise TypeError("target must hold integer ids (got %s)" % t.dtype)
-    if t.shape[0] < n * k_nn:
-        raise ValueError("target has %d ids for %d vertices of %d neighbours" % (t.shape[0], n, k_nn))
-    _dtype(xyz)
-    dev = _device_of(xyz, target)
-    if not torch.is_tensor(t):
-        t = torch.from_numpy(np.ascontiguousarray(t[:n * k_nn], dtype=np.int64))
-    t = t[:n * k_nn].to(device=dev, dtype=torch.int64).contiguous()
-    xyz = _xyz(xyz, dev)
+    n_ids = math.prod(check_ints(target, "target"))
+    if n_ids < n * k_nn:
+        raise ValueError("target has %d ids for %d vertices of %d neighbours" % (n_ids, n, k_nn))
+    check_dtype(xyz, "xyz", "float32")
+    dev = device_of(xyz, target)
+    t = target.reshape(-1) if torch.is_tensor(target) else np.asarray(target).reshape(-1)
+    t = on_device(t[:n * k_nn], dev, int64=True)
+    xyz = on_device(xyz, dev)
     with torch.cuda.device(dev):
         out, status = ops.geof(xyz, t, k_nn)
         if int(status.item()) & 2:

@@ -25,17 +25,11 @@ import numpy as np
 import torch
 
 from . import ops
+from ._inputs import device_of
 
 __all__ = ["compute_dist", "compute_loss", "compute_partition", "compute_weight_loss", "compute_weights_SEAL",
            "compute_weights_XPART", "relax_edge_binary", "compute_boundary_recall", "compute_boundary_precision",
            "perfect_prediction", "partition_edge_weight", "boundary_counts", "loss_kinds"]
-
-
-def _device(*candidates):
-    for c in candidates:
-        if torch.is_tensor(c) and c.is_cuda:
-            return c.device
-    return torch.device("cuda", torch.cuda.current_device())
 
 
 def _edges(edg, n_ver, dev):
@@ -177,7 +171,7 @@ def compute_weights_SEAL(pred_components, pred_in_component, objects, edg_source
                          transition_factor):
     """float32 CUDA [E] — ref: losses.py:119-128 (w per component = size - mode frequency, by a device sort of
     (component, object) pairs)."""
-    dev = _device(objects, is_transition, edg_source)
+    dev = device_of(objects, is_transition, edg_source)
     pic = _int64(pred_in_component, dev)
     V = pic.numel()
     w, _ = ops.lp_seal(_edges(edg_source, V, dev), _edges(edg_target, V, dev), _mask(is_transition, dev), pic,
@@ -190,7 +184,7 @@ def compute_weights_XPART(pred_components, pred_in_component, objects, edg_sourc
     """float32 CUDA [E] — ref: losses.py:130-166: connected components of the edges that are neither true nor
     predicted transitions, then 1 + min(|c1|, |c2|) / #edges(c1, c2) * transition_factor on every transition edge,
     by a radix sort of the unordered component pairs instead of the reference's loop over them."""
-    dev = _device(is_transition, edg_source, pred_in_component)
+    dev = device_of(is_transition, edg_source, pred_in_component)
     pic = _int64(pred_in_component, dev)
     V = pic.numel()
     return ops.lp_xpart(_edges(edg_source, V, dev), _edges(edg_target, V, dev), _mask(is_transition, dev), pic, V,
@@ -203,7 +197,7 @@ def compute_weight_loss(args, embeddings, objects, edg_source, edg_target, is_tr
     skips cut pursuit; without it the schemes that need one (and return_partition) call compute_partition."""
     if partition is None and (args.loss_weight in ("seal", "crosspartition") or return_partition):
         partition = compute_partition(args, embeddings, edg_source, edg_target, diff, xyz)
-    dev = diff.device if torch.is_tensor(diff) and diff.is_cuda else _device(embeddings, is_transition)
+    dev = device_of(diff, embeddings, is_transition)
     is_tr = _mask(is_transition, dev)
     E = is_tr.numel()
     if args.loss_weight == "none":
@@ -233,7 +227,7 @@ def relax_edge_binary(edg_binary, edg_source, edg_target, n_ver, tolerance):
     anything else uint8): each round marks the endpoints of the set edges, then sets edge 0 if some edge's
     source is unmarked and edge 1 if some edge's source is marked (losses.py:184 indexes with the uint8 marks),
     then every edge whose target is marked (:185)."""
-    dev = _device(edg_binary, edg_source)
+    dev = device_of(edg_binary, edg_source)
     is_bool = (edg_binary.dtype == torch.bool) if torch.is_tensor(edg_binary) else np.asarray(edg_binary).dtype == bool
     relaxed = _mask(edg_binary, dev).clone()
     src, tgt = _edges(edg_source, n_ver, dev), _edges(edg_target, n_ver, dev)
@@ -246,7 +240,7 @@ def relax_edge_binary(edg_binary, edg_source, edg_target, n_ver, tolerance):
 def boundary_counts(truth, pred):
     """(numerator, denominator) of 100 * ((truth == pred) * truth).sum() / truth.sum() for 0/1 masks, counted on
     the device; only these two integers come back."""
-    dev = _device(truth, pred)
+    dev = device_of(truth, pred)
     c = ops.lp_count(_mask(truth, dev), _mask(pred, dev)).cpu().numpy()
     return int(c[0]), int(c[1])
 
@@ -270,7 +264,7 @@ def perfect_prediction(components, labels):
     """Majority label of every point's component (ref: partition/provider.py:689-695): per component the int64
     sum of labels[:, 1:], the first maximum wins (numpy's argmax), scattered to the points.  int64 CUDA [V]; pass
     `.cpu().numpy()` to a host ConfusionMatrix."""
-    dev = _device(labels)
+    dev = device_of(labels)
     lab = _int64(labels, dev)
     sizes = np.asarray([len(c) for c in components], dtype=np.int64)
     ptr = np.zeros(len(components) + 1, dtype=np.int64)

@@ -29,8 +29,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .spg_geometry import _device_of, _dtype, _n_rows, _xyz
-from .spg_sp_graph import _check_ints, _ints
+from ._inputs import check_dtype, check_ints, device_of, n_points, on_device
 
 __all__ = ["prune", "to_numpy"]
 
@@ -44,23 +43,9 @@ def _count(v, name):
     return int(v)
 
 
-def _check_rgb(rgb, n):
-    dt, shape = (rgb.dtype, tuple(rgb.shape)) if torch.is_tensor(rgb) else (np.asarray(rgb).dtype, np.shape(rgb))
-    if dt not in (torch.uint8, np.uint8):
-        raise TypeError("rgb must be uint8 (got %s)" % dt)
-    if tuple(shape) != (n, 3):
-        raise ValueError("rgb has shape %s for %d points (want [n, 3])" % (tuple(shape), n))
-
-
-def _rgb(rgb, device):
-    if torch.is_tensor(rgb):
-        return rgb.to(device).contiguous()
-    return torch.from_numpy(np.ascontiguousarray(rgb)).to(device)
-
-
 def _check_ids(a, name, n):
     """A label or object array read by the reference: integers, one per point."""
-    shape = _check_ints(a, name)
+    shape = check_ints(a, name)
     if len(shape) == 0 or shape[0] != n or int(np.prod(shape)) != n:
         raise ValueError("%s has shape %s for %d points" % (name, tuple(shape), n))
 
@@ -74,10 +59,10 @@ def prune(xyz, voxel_size, rgb, labels, objects, n_labels, n_objects, chunk_rows
     negative n_labels / n_objects / chunk_rows, row-count mismatches of the arrays read.  TypeError: xyz not float32,
     rgb not uint8, non-integer labels or objects.  IndexError: a label outside [0, n_labels] or an object outside
     [0, n_objects]."""
-    n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
+    n = n_points(np.shape(xyz))
     if n == 0:
         raise ValueError("prune needs at least one point")
-    _dtype(xyz)
+    check_dtype(xyz, "xyz", "float32")
     n_labels = _count(n_labels, "n_labels")
     n_objects = _count(n_objects, "n_objects")
     chunk_rows = _count(chunk_rows, "chunk_rows")
@@ -89,16 +74,18 @@ def prune(xyz, voxel_size, rgb, labels, objects, n_labels, n_objects, chunk_rows
         raise ValueError("voxel_size must be finite and > 0 (got %r)" % (voxel_size,))
     with_labels = n_labels > 0
     with_objects = with_labels and n_objects > 0
-    _check_rgb(rgb, n)
+    rgb_shape = check_dtype(rgb, "rgb", "uint8")
+    if rgb_shape != (n, 3):
+        raise ValueError("rgb has shape %s for %d points (want [n, 3])" % (rgb_shape, n))
     if with_labels:
         _check_ids(labels, "labels", n)
     if with_objects:
         _check_ids(objects, "objects", n)
-    dev = _device_of(xyz, rgb, labels, objects)
-    xyz = _xyz(xyz, dev)
-    rgb = _rgb(rgb, dev)
-    lab = _ints(labels, "labels", dev).reshape(-1) if with_labels else None
-    obj = _ints(objects, "objects", dev).reshape(-1) if with_objects else None
+    dev = device_of(xyz, rgb, labels, objects)
+    xyz = on_device(xyz, dev)
+    rgb = on_device(rgb, dev)
+    lab = on_device(labels, dev, int64=True).reshape(-1) if with_labels else None
+    obj = on_device(objects, dev, int64=True).reshape(-1) if with_objects else None
     with torch.cuda.device(dev):
         ws = ops.prune_workspace(n, chunk_rows, dev)
         words = [int(v) for v in ops.prune_bounds(xyz, chunk_rows, voxel, lab, n_labels, obj, n_objects, ws).cpu()]

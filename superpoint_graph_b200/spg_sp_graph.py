@@ -25,48 +25,9 @@ import numpy as np
 import torch
 
 from . import ops
-from .spg_geometry import _device_of, _dtype, _n_rows, _xyz
+from ._inputs import check_dtype, check_ints, device_of, n_points, on_device, simplices_on
 
 __all__ = ["compute_sp_graph", "to_numpy"]
-
-
-def _check_ints(a, name):
-    """The shape of an integer array or tensor; other dtypes are refused."""
-    if torch.is_tensor(a):
-        if a.dtype.is_floating_point or a.dtype.is_complex or a.dtype == torch.bool:
-            raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
-        return tuple(a.shape)
-    a = np.asarray(a)
-    if a.dtype.kind not in "iu":
-        raise TypeError("%s must hold integers (got %s)" % (name, a.dtype))
-    return a.shape
-
-
-def _ints(a, name, device):
-    """An integer array or tensor as a contiguous int64 tensor on the device; other dtypes are refused."""
-    _check_ints(a, name)
-    if torch.is_tensor(a):
-        return a.to(device=device, dtype=torch.int64).contiguous()
-    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(device)
-
-
-def _simplices(simplices, xyz, device):
-    if simplices is None:
-        from scipy.spatial import Delaunay  # host triangulation; scipy is imported only when it is needed
-
-        host = xyz.cpu().numpy() if torch.is_tensor(xyz) else np.asarray(xyz)
-        simplices = Delaunay(host).simplices
-    shape = tuple(simplices.shape)
-    if len(shape) != 2 or shape[1] != 4:
-        raise ValueError("simplices must be [T, 4] (got shape %s)" % (shape,))
-    if torch.is_tensor(simplices):
-        if simplices.dtype == torch.int32:
-            return simplices.to(device).contiguous()
-        return _ints(simplices, "simplices", device)
-    s = np.asarray(simplices)
-    if s.dtype == np.int32:
-        return torch.from_numpy(np.ascontiguousarray(s)).to(device)
-    return _ints(s, "simplices", device)
 
 
 def _label_mode(labels, n, n_labels):
@@ -74,7 +35,7 @@ def _label_mode(labels, n, n_labels):
     more than one column; else 1 (the histogram of the values 0..n_labels)."""
     if len(labels) <= 1:
         return 0
-    shape = _check_ints(labels, "labels")
+    shape = check_ints(labels, "labels")
     if shape[0] != n:
         raise ValueError("labels has %d rows for %d points" % (shape[0], n))
     if len(shape) > 1 and shape[1] > 1:
@@ -91,22 +52,22 @@ def compute_sp_graph(xyz, d_max, in_component, components, labels, n_labels, sim
     ValueError: a non-finite coordinate, a negative or empty component id below max + 1, len(components) other than
     max(in_component) + 1, a label histogram without n_labels + 1 columns.  TypeError: xyz not float32, non-integer
     ids, labels or simplices.  IndexError: a simplex id outside [0, n)."""
-    n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
+    n = n_points(np.shape(xyz))
     if n == 0:
         raise ValueError("compute_sp_graph needs at least one point")
-    _dtype(xyz)
+    check_dtype(xyz, "xyz", "float32")
     n_labels = int(n_labels)
-    shape = _check_ints(in_component, "in_component")
+    shape = check_ints(in_component, "in_component")
     if len(shape) != 1 or shape[0] != n:
         raise ValueError("in_component has shape %s for %d points" % (shape, n))
     label_mode = _label_mode(labels, n, n_labels)
-    dev = _device_of(xyz, in_component, simplices)
+    dev = device_of(xyz, in_component, simplices)
     host_xyz = xyz
-    xyz = _xyz(xyz, dev)
-    comp = _ints(in_component, "in_component", dev)
+    xyz = on_device(xyz, dev)
+    comp = on_device(in_component, dev, int64=True)
     lab = None
     if label_mode:
-        lab = _ints(labels, "labels", dev)
+        lab = on_device(labels, dev, int64=True)
         lab = lab.reshape(-1) if label_mode == 1 else lab
     with torch.cuda.device(dev):
         n_com, status = (int(v) for v in ops.sp_scan(xyz, comp).cpu())
@@ -118,7 +79,12 @@ def compute_sp_graph(xyz, d_max, in_component, components, labels, n_labels, sim
             raise ValueError("%d components for %d points: some component holds no point" % (n_com, n))
         if len(components) != n_com:
             raise ValueError("components has %d entries for max(in_component) + 1 = %d" % (len(components), n_com))
-        tets = _simplices(simplices, host_xyz, dev)
+        if simplices is None:
+            from scipy.spatial import Delaunay  # host triangulation; scipy is imported only when it is needed
+
+            host = host_xyz.cpu().numpy() if torch.is_tensor(host_xyz) else np.asarray(host_xyz)
+            simplices = Delaunay(host).simplices
+        tets = simplices_on(simplices, dev)
         sp, sp_status = ops.sp_points(xyz, comp, n_com, lab, label_mode, n_labels)
         offsets, e_status = ops.sp_edges_count(comp, tets)
         if int(sp_status.item()) & 8:

@@ -26,9 +26,8 @@ import numpy as np
 import torch
 
 from . import ops, spg_delaunay, spg_geometry
+from ._inputs import check_dtype, check_ints, device_of, n_points, on_device, simplices_on
 from .spg_cut_pursuit import Components
-from .spg_geometry import _device_of, _n_rows, _xyz
-from .spg_sp_graph import _check_ints, _ints, _simplices
 
 __all__ = ["compute_graph_nn_2", "connected_comp", "compute_structure", "inpainting_problem", "to_numpy",
            "as_read_structure"]
@@ -54,10 +53,10 @@ def compute_graph_nn_2(xyz, k_nn1, k_nn2, voronoi=0.0, simplices=None):
     dev = graph["target"].device
     vor = float(np.float32(voronoi))
     with torch.cuda.device(dev):
-        x = _xyz(xyz, dev)
+        x = on_device(xyz, dev)
         if simplices is None:
             simplices = spg_delaunay.delaunay(x)
-        simp = _simplices(simplices, x, dev)
+        simp = simplices_on(simplices, dev)
         counts, status = ops.st_vor_count(x, simp, vor)
         _raise_ids(status, "simplices")
         n_kept = int(counts[-1].item())
@@ -68,9 +67,9 @@ def compute_graph_nn_2(xyz, k_nn1, k_nn2, voronoi=0.0, simplices=None):
 
 
 def _edge_ids(a, name, dev):
-    if len(_check_ints(a, name)) != 1:
+    if len(check_ints(a, name)) != 1:
         raise ValueError("%s must be 1-D" % name)
-    return _ints(a, name, dev)
+    return on_device(a, dev, int64=True)
 
 
 def connected_comp(n_ver, source, target, active_edg, cutoff=0):
@@ -93,7 +92,7 @@ def connected_comp(n_ver, source, target, active_edg, cutoff=0):
     dt = active_edg.dtype if torch.is_tensor(active_edg) else np.asarray(active_edg).dtype
     if dt not in (torch.uint8, torch.int8, torch.bool, np.uint8, np.int8, np.bool_):
         raise TypeError("active_edg must be uint8, int8 or bool (got %s)" % dt)
-    dev = _device_of(source, target, active_edg)
+    dev = device_of(source, target, active_edg)
     with torch.cuda.device(dev):
         src = _edge_ids(source, "source", dev)
         tgt = _edge_ids(target, "target", dev)
@@ -119,17 +118,17 @@ def _field(args, name):
 
 
 def _histogram(a, name, n, dev):
-    shape = _check_ints(a, name)
+    shape = check_ints(a, name)
     if len(shape) != 2 or shape[0] != n or shape[1] < 1:
         raise ValueError("%s must be a [%d, C] histogram (got shape %s)" % (name, n, tuple(shape)))
-    return _ints(a, name, dev)
+    return on_device(a, dev, int64=True)
 
 
 def _per_vertex(a, name, n, dev):
-    shape = _check_ints(a, name)
+    shape = check_ints(a, name)
     if tuple(shape) not in ((n,), (n, 1)):
         raise ValueError("%s must hold one integer per vertex (got shape %s)" % (name, tuple(shape)))
-    return _ints(a, name, dev).reshape(-1)
+    return on_device(a, dev, int64=True).reshape(-1)
 
 
 def _transitions(lab, graph_nn, mode=ops.ST_DIFFERENT):
@@ -147,7 +146,8 @@ def inpainting_problem(labels, graph_nn):
     src = graph_nn["source"]
     dev = src.device
     with torch.cuda.device(dev):
-        lab = _ints(labels, "labels", dev)
+        check_ints(labels, "labels")
+        lab = on_device(labels, dev, int64=True)
         if lab.dim() != 2 or lab.shape[1] < 2:
             raise ValueError("labels must be a [n, C] histogram with C >= 2 (got shape %s)" % (tuple(lab.shape),))
         hard, node_weight = ops.st_argmax(lab, 1, 1, zero_empty=True, want_weight=True)
@@ -198,7 +198,7 @@ def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True
     k_adj, k_local = _field(args, "k_nn_adj"), _field(args, "k_nn_local")
     voronoi, want_geof, plane_model = (_field(args, "use_voronoi"), _field(args, "compute_geof"),
                                        _field(args, "plane_model"))
-    n = _n_rows(tuple(xyz.shape) if torch.is_tensor(xyz) else np.shape(xyz))
+    n = n_points(np.shape(xyz))
     if dataset == "sema3d" and labels is not None and objects is None:
         raise NotImplementedError("sema3d with labels needs libcp.cutpursuit2 (node-weighted cut pursuit), which is "
                                   "not computed on the device: pass its objects as objects=, see inpainting_problem")
@@ -206,12 +206,14 @@ def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True
         raise ValueError("s3dis needs objects")
     if dataset == "vkitti" and labels is None:
         raise ValueError("vkitti needs labels")
-    dev = _device_of(xyz, rgb, labels, objects)
+    dev = device_of(xyz, rgb, labels, objects)
     with torch.cuda.device(dev):
-        x = _xyz(xyz, dev)
-        rgb_d = rgb.to(dev) if torch.is_tensor(rgb) else torch.from_numpy(np.ascontiguousarray(rgb)).to(dev)
+        check_dtype(xyz, "xyz", "float32")
+        x = on_device(xyz, dev)
+        rgb_d = on_device(rgb, dev)
         if dataset == "s3dis":
-            lab = _ints(labels, "labels", dev)
+            check_ints(labels, "labels")
+            lab = on_device(labels, dev, int64=True)
             obj = (ops.st_argmax(_histogram(objects, "objects", n, dev), 1, 1)[0] if pruned
                    else _per_vertex(objects, "objects", n, dev))
         elif dataset == "vkitti":
@@ -220,7 +222,8 @@ def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True
             lab = torch.zeros(1, dtype=torch.int64, device=dev)
             obj = torch.zeros(1, dtype=torch.int64, device=dev)
         else:
-            lab = _ints(labels, "labels", dev)
+            check_ints(labels, "labels")
+            lab = on_device(labels, dev, int64=True)
             obj = _per_vertex(objects, "objects", n, dev)
         graph_nn, target2 = compute_graph_nn_2(x, k_adj, k_local, voronoi=voronoi, simplices=simplices)
         if dataset == "vkitti":
