@@ -969,6 +969,38 @@ int spg_st_gather_rows(const void* src, int64_t n_rows, int64_t row_bytes, const
 int spg_st_points(const float* xyz, int64_t n, const uint32_t* bounds, int plane, double c0, double c1, double b,
                   float* elevation, float* xyn, uint8_t* low, float* geof, spg_stream_t stream);
 
+/* ---------------------------------------------------------------- superpoint graph batch builder
+ * loader's sub-graph selection + eccpc_collate / GraphConvInfo.set_batch, one graph of the batch per call.
+ * ref: learning/spg.py:114-143,178-193, learning/ecc/GraphConvInfo.py:33-69
+ *
+ * batch_select: src / tgt [E] (int32, the file's edge order); the undirected adjacency is the spg_graph_build
+ * views of the file's stably target-sorted edges (tgt_rowptr [n + 1], in_src = its idxn [E], src_rowptr
+ * [n + 1], src_perm [E], edge_tgt [E]); sizes [n] (int64) the vertex attribute s.  perm [n] (new id of every
+ * vertex, NULL: identity).  centres [n_centres] (new ids; NULL: every vertex kept) start a BFS of depth `order`
+ * ignoring edge directions.  cut > 0 keeps the prefix, in increasing new id, of the kept vertices whose running
+ * count of s >= minpts is <= cut (k_big_enough).  Outputs: new_index [n] = sub-graph id of every vertex or -1,
+ * edge_pos [E + 1] = exclusive scan of the kept-edge flags, out [2 + n] = (kept vertices, kept edges, the kept
+ * original ids in sub-graph order).  Workspace from spg_batch_select_workspace, 256-byte aligned.          */
+int spg_batch_select_workspace(int64_t n_ver, int64_t n_edges, int64_t* bytes);
+int spg_batch_select(const int32_t* src, const int32_t* tgt, int64_t n_ver, int64_t n_edges,
+                     const int32_t* tgt_rowptr, const int32_t* in_src, const int32_t* src_rowptr,
+                     const int32_t* src_perm, const int32_t* edge_tgt, const int64_t* sizes, const int32_t* perm,
+                     const int32_t* centres, int64_t n_centres, int order, int64_t minpts, int64_t cut,
+                     int32_t* new_index, int32_t* edge_pos, int32_t* out, void* workspace, int64_t workspace_bytes,
+                     spg_stream_t stream);
+/* batch_edges: the graph's slice of the collated batch.  The kept edges in file order, stably sorted by new
+ * target; idxn_out / tgt_out [kE] = vertex_offset + new (source, target), degs_out [n_kept] = in-degrees,
+ * feats_out [kE, n_feats] = edge_feats rows, targets_out [n_kept, n_target_cols] = targets rows of kept
+ * (the original ids, batch_select's out + 2).  Workspace from spg_batch_edges_workspace.
+ * ref: learning/spg.py:183-185, learning/ecc/GraphConvInfo.py:48-69                                       */
+int spg_batch_edges_workspace(int64_t n_kept, int64_t n_kept_edges, int64_t* bytes);
+int spg_batch_edges(const int32_t* src, const int32_t* tgt, int64_t n_edges, const int32_t* new_index,
+                    const int32_t* edge_pos, const int32_t* kept, int64_t n_kept, int64_t n_kept_edges,
+                    int64_t vertex_offset, const float* edge_feats, int64_t n_feats, const int64_t* targets,
+                    int64_t n_target_cols, int64_t* idxn_out, int64_t* tgt_out, int64_t* degs_out,
+                    float* feats_out, int64_t* targets_out, void* workspace, int64_t workspace_bytes,
+                    spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -117,6 +117,8 @@ enum KernelId {
     K_ST_LABELS,
     K_ST_SELECT,
     K_ST_POINTS,
+    K_SB_SELECT,
+    K_SB_EDGES,
     K_COUNT
 };
 

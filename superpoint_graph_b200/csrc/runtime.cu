@@ -40,7 +40,7 @@ static const char* kKernelNames[K_COUNT] = {
     "dt_setup",          "dt_init",            "dt_nominate",         "dt_grow",
     "dt_check",          "dt_commit",          "dt_relocate",         "dt_output",
     "st_vor",            "st_cc",              "st_labels",           "st_select",
-    "st_points",
+    "st_points",         "sb_select",          "sb_edges",
 };
 
 struct Record {

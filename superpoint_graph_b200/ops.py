@@ -1748,3 +1748,33 @@ def st_points(xyz, bounds, plane=None, elevation=None, xyn=None, low=None, geof=
     c0, c1, b = (0.0, 0.0, 0.0) if plane is None else plane
     _lib.call("spg_st_points", xyz, xyz.shape[0], bounds, int(plane is not None), float(c0), float(c1), float(b),
               elevation, xyn, low, geof, _lib.current_stream())
+
+
+# ------------------------------------------------------------- superpoint graph batch builder
+
+def batch_select(src, tgt, adjacency, sizes, perm, centres, order, minpts, cut):
+    """Sub-graph selection of one resident graph (see spg_batch_select).  adjacency: the spg_graph_build views
+    (EccGraph.to(device)) of its target-sorted edges.  Returns (new_index int32 [n], edge_pos int32 [E + 1],
+    out int32 [2 + n] = kept vertices, kept edges, kept original ids)."""
+    _need_cuda(src, tgt, sizes, perm, centres)
+    n, E = sizes.numel(), src.numel()
+    i32 = dict(dtype=torch.int32, device=sizes.device)
+    new_index, edge_pos, out = torch.empty(n, **i32), torch.empty(E + 1, **i32), torch.empty(2 + n, **i32)
+    ws = _workspace("spg_batch_select_workspace", sizes.device, n, E)
+    _lib.call("spg_batch_select", src, tgt, n, E, adjacency["tgt_rowptr"], adjacency["idxn"],
+              adjacency["src_rowptr"], adjacency["src_perm"], adjacency["edge_tgt"], sizes, perm, centres,
+              0 if centres is None else centres.numel(), int(order), int(minpts), int(cut), new_index, edge_pos, out,
+              ws, ws.numel(), _lib.current_stream())
+    return new_index, edge_pos, out
+
+
+def batch_edges(src, tgt, new_index, edge_pos, kept, n_kept, n_kept_edges, vertex_offset, edge_feats, targets,
+                idxn_out, tgt_out, degs_out, feats_out, targets_out):
+    """One graph's slice of the collated batch (see spg_batch_edges); every output is that slice."""
+    _need_cuda(src, tgt, new_index, edge_pos, kept, edge_feats, targets, idxn_out, tgt_out, degs_out, feats_out,
+               targets_out)
+    assert edge_feats.dtype == torch.float32 and targets.dtype == torch.int64
+    ws = _workspace("spg_batch_edges_workspace", src.device, n_kept, n_kept_edges)
+    _lib.call("spg_batch_edges", src, tgt, src.numel(), new_index, edge_pos, kept, int(n_kept), int(n_kept_edges),
+              int(vertex_offset), edge_feats, edge_feats.shape[1], targets, targets.shape[1], idxn_out, tgt_out,
+              degs_out, feats_out, targets_out, ws, ws.numel(), _lib.current_stream())

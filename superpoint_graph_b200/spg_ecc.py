@@ -79,6 +79,18 @@ class GraphConvInfo(object):
         gi._edge_indexes = torch.stack([gi._idxn, tgt])
         return gi
 
+    @classmethod
+    def from_device_arrays(cls, edge_index, degrees, edgefeats):
+        """Builds the info object from a collated batch already on the device: edge_index int64 [2, E] (source
+        and target of every edge, sorted by target), degrees int64 [N], edgefeats [E, F].  The state is the one
+        cuda() leaves (idxn, degrees and edge features on the device, the kernels' CSR views built by
+        spg_graph_build), so a later cuda() or set_info(..., cuda=True) changes nothing."""
+        gi = cls()
+        gi._idxn, gi._degrees, gi._degrees_gpu = edge_index[0], degrees, degrees
+        gi._edgefeats, gi._edge_indexes = edgefeats, edge_index
+        gi._graph = ops.EccGraph.from_device(gi._idxn, degrees, n_in=int(degrees.numel()), check=False)
+        return gi
+
     def graph(self):
         """The CSR bundle the kernels read (built once per batch from idxn/degs: on the device by cuda(),
         else on first use from the host arrays)."""

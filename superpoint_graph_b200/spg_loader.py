@@ -17,7 +17,7 @@ import random
 import numpy as np
 import torch
 
-from . import ops
+from . import _inputs, ops
 
 _ATTRIBS = (("xyz", (0, 1, 2)), ("rgb", (3, 4, 5)), ("e", (6,)), ("lpsv", (7, 8, 9, 10)),
             ("XYZ", (11, 12, 13)))
@@ -157,3 +157,154 @@ def load_superpoints(store, fname, sp_ids, args, train, test_seed_offset=0, devi
             torch.from_numpy(np.stack(noise)).to(dev) if noise else None,
             0.01 if (jitter and device_rng) else 0.0, 0.05, seed, clouds, diam)
     return np.array(flags), clouds, diam
+
+
+class GraphStore(object):
+    """Superpoint graphs of one or more files, resident on the device (the graph half of the reference's
+    `loader`, learning/spg.py:106-143).
+
+    `add(node_gt, node_gt_size, edges, edge_feats, name)` takes spg_reader's tuple in its order (after
+    scaler01); `finalize(device)` uploads once.  Kept per vertex: the target row [node_gt | node_gt_size] (int64,
+    spg_to_igraph's 't') and s = node_gt_size.sum(1) (int64); per edge: source and target (int32, file order) and
+    the feature row (float32); per file: the spg_graph_build views of its stably target-sorted edges, whose target
+    and source CSRs together are the undirected adjacency the neighbourhood BFS walks.  No batch writes to them.
+    `add` validates on the host and raises as numpy would: IndexError for an edge id out of range, ValueError for
+    inconsistent lengths, files of 2^31 vertices or more or a name added twice; TypeError for edge features that are
+    not float32."""
+
+    def __init__(self):
+        self._host, self._files = {}, {}
+        self.device = None
+
+    def add(self, node_gt, node_gt_size, edges, edge_feats, name):
+        if self.device is not None:
+            raise RuntimeError("GraphStore.add after finalize")
+        if name in self._host:
+            raise ValueError("%s: a graph of this name was added already" % (name,))
+        node_gt, node_gt_size = np.asarray(node_gt), np.asarray(node_gt_size)
+        n = node_gt.shape[0]
+        if n >= 2 ** 31:
+            raise ValueError("%s: %d vertices; files of 2^31 vertices or more are not supported" % (name, n))
+        if node_gt.ndim != 2 or node_gt_size.ndim != 2 or node_gt_size.shape[0] != n:
+            raise ValueError("%s: node_gt %s and node_gt_size %s are not [n, 1] and [n, C]"
+                             % (name, node_gt.shape, node_gt_size.shape))
+        _inputs.check_ints(edges, "edges")
+        edges = np.asarray(edges)
+        if edges.ndim != 2 or edges.shape[1] != 2:
+            raise ValueError("%s: edges must be [E, 2] (got shape %s)" % (name, edges.shape))
+        fshape = _inputs.check_dtype(edge_feats, "edge_feats", "float32")
+        if len(fshape) != 2 or fshape[0] != edges.shape[0]:
+            raise ValueError("%s: edge_feats has shape %s for %d edges" % (name, tuple(fshape), edges.shape[0]))
+        if edges.size and (int(edges.min()) < 0 or int(edges.max()) >= n):
+            bad = int(edges.max()) if int(edges.max()) >= n else int(edges.min())
+            raise IndexError("%s: index %d is out of bounds for axis 0 with size %d" % (name, bad, n))
+        self._host[name] = dict(
+            n=n, targets=np.concatenate([node_gt, node_gt_size], axis=1).astype(np.int64),
+            s=node_gt_size.sum(1).astype(np.int64), src=edges[:, 0].astype(np.int32),
+            tgt=edges[:, 1].astype(np.int32), feats=np.ascontiguousarray(edge_feats))
+        return self
+
+    def finalize(self, device):
+        """Uploads every added file and builds its adjacency on the device."""
+        device = torch.device(device)
+        for name, h in self._host.items():
+            order = np.argsort(h["tgt"], kind="stable")
+            up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
+            f = dict(name=name, n=h["n"], E=h["src"].size, targets=up(h["targets"]), s=up(h["s"]), src=up(h["src"]),
+                     tgt=up(h["tgt"]), feats=up(h["feats"]))
+            degs = up(np.bincount(h["tgt"], minlength=h["n"]).astype(np.int64))
+            idxn = up(h["src"][order].astype(np.int64))
+            views = ops.EccGraph.from_device(idxn, degs, n_in=h["n"], check=False).to(idxn.device)
+            f["adjacency"] = {k: views[k] for k in ops.EccGraph.GRAPH_FIELDS}
+            self._files[name] = f
+        self._host = {}
+        self.device = device
+        return self
+
+    def file(self, name):
+        if self.device is None:
+            raise RuntimeError("GraphStore.finalize(device) has not been called")
+        return self._files[name]
+
+
+def graph_draws(n, train, args):
+    """The sampling draws of `loader` for a graph of n vertices (ref: learning/spg.py:134-143), from Python's
+    global `random` in the reference's order: the permutation (perm[i] = new id of vertex i) when
+    0 < hardcutoff < n, then the centres (new ids) when 0 < nneigh < n.  Returns (perm or None, centres or None,
+    cut): cut > 0 is k_big_enough's k, which keeps everything unless it is below the sub-graph's size."""
+    perm = centres = None
+    if not train:
+        return perm, centres, 0
+    hc, nn = int(args.spg_augm_hardcutoff), int(args.spg_augm_nneigh)
+    if 0 < hc < n:
+        perm = list(range(n))
+        random.shuffle(perm)
+    if 0 < nn < n:
+        centres = random.sample(range(n), k=nn)
+    return perm, centres, max(hc, 0)
+
+
+def load_batch(gstore, cstore, names, train, args, test_seed_offset=0):
+    """`loader(entry, train, args, db_path, test_seed_offset)` for every name, then `eccpc_collate`
+    (ref: learning/spg.py:130-193).  Returns (targets, GIs, (clouds_meta, clouds_flag, clouds, clouds_global))
+    with targets int64 [N, 2 + C], clouds and clouds_global on the device, GIs = [GraphConvInfo] whose idxn,
+    degs_gpu and edgefeats are on the device with its kernel views built.
+
+    Graph by graph, as the reference: the sampling draws, the selection on the device, one read-back of the counts
+    and kept ids (none when the whole graph is kept; one copy of the whole [2 + n] word array, so one
+    synchronisation, where reading the count first would take two), then load_superpoints' cloud draws for graphs with edges.
+    Graphs without edges are dropped; the collate's exceptions are the reference's (RuntimeError when no graph
+    has an edge, TypeError when the first has none or a graph with edges has no cloud)."""
+    from .spg_ecc import GraphConvInfo
+
+    dev = gstore.device
+    picks = []
+    for name in names:
+        f = gstore.file(name)
+        n = f["n"]
+        perm, centres, cut = graph_draws(n, train, args)
+        if perm is None and centres is None and not 0 < cut < n:
+            new_index = edge_pos = kept_dev = None
+            n_kept, n_edges, ids = n, f["E"], list(range(n))
+        else:
+            to_dev = lambda a: None if a is None else torch.tensor(a, dtype=torch.int32).to(dev)
+            new_index, edge_pos, out = ops.batch_select(
+                f["src"], f["tgt"], f["adjacency"], f["s"], to_dev(perm), to_dev(centres),
+                int(args.spg_augm_order), int(args.ptn_minpts), cut)
+            host = out.cpu().numpy()
+            n_kept, n_edges = int(host[0]), int(host[1])
+            ids, kept_dev = host[2:2 + n_kept].tolist(), out[2:2 + n_kept]
+        clouds = load_superpoints(cstore, name, ids, args, train, test_seed_offset) if n_edges else None
+        picks.append((f, new_index, edge_pos, kept_dev, n_kept, n_edges, ids, clouds))
+    kept = [p for p in picks if p[5]]
+    if not kept:
+        raise RuntimeError("torch.cat(): expected a non-empty list of Tensors")
+    if not picks[0][5]:
+        raise TypeError("object of type 'NoneType' has no len()")
+    if any(p[7][1].shape[0] == 0 for p in kept):
+        raise TypeError("expected np.ndarray (got list)")
+    feats_w = {p[0]["feats"].shape[1] for p in kept}
+    cols = {p[0]["targets"].shape[1] for p in kept}
+    if len(feats_w) > 1 or len(cols) > 1:
+        raise ValueError("the graphs of a batch have different edge-feature or target widths")
+    N, E = sum(p[4] for p in kept), sum(p[5] for p in kept)
+    i64 = dict(dtype=torch.int64, device=dev)
+    edge_index, degs = torch.empty((2, E), **i64), torch.empty(N, **i64)
+    edgefeats = torch.empty((E, feats_w.pop()), dtype=torch.float32, device=dev)
+    targets = torch.empty((N, cols.pop()), **i64)
+    vo = eo = 0
+    for f, new_index, edge_pos, kept_ids, n_kept, n_edges, _, _ in kept:
+        if new_index is None:
+            i32 = dict(dtype=torch.int32, device=dev)
+            new_index = kept_ids = torch.arange(n_kept, **i32)
+            edge_pos = torch.arange(n_edges + 1, **i32)
+        ops.batch_edges(f["src"], f["tgt"], new_index, edge_pos, kept_ids, n_kept, n_edges, vo, f["feats"],
+                        f["targets"], edge_index[0, eo:eo + n_edges], edge_index[1, eo:eo + n_edges],
+                        degs[vo:vo + n_kept], edgefeats[eo:eo + n_edges], targets[vo:vo + n_kept])
+        vo, eo = vo + n_kept, eo + n_edges
+    gi = GraphConvInfo.from_device_arrays(edge_index, degs, edgefeats)
+    clouds_meta = ["{}.{:d}".format(p[0]["name"], v) for p in kept for v in p[6]]
+    clouds_flag = torch.from_numpy(np.concatenate([p[7][0] for p in kept]))
+    clouds = torch.cat([p[7][1] for p in kept], 0)
+    clouds_global = torch.cat([p[7][2] for p in kept], 0)
+    return targets, [gi], (clouds_meta, clouds_flag, clouds, clouds_global)
