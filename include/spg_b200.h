@@ -838,10 +838,17 @@ int spg_prune_reduce(const float* xyz, const uint8_t* rgb, const int64_t* labels
  * active (uint8 [n_edges]), value, c0, c1 (float64 [n, dim]), cs, ct (float32 [n]), ecap (float32 [n_edges]),
  * members, offsets (int32), words (int64), dwords (float64), partner (int32 [n]), res (int64 [2 n_edges]: the
  * residual fixed-point capacities of the arcs), excess, rt (int64 [n]: excess and residual sink capacity), arc_off
- * (int32 [n + 1]), arc_dst, arc_rev, arc_edge (int32 [2 n_edges]: head, reverse arc and listed edge of every arc).
+ * (int32 [n + 1]), arc_dst, arc_rev, arc_edge (int32 [2 n_edges]: head, reverse arc and listed edge of every arc),
+ * nw (float32 [n]: the vertex weights) and cw (float64 [n]: the component weights, sum of nw, as of the last value
+ * computation).
  *
  * spg_cp_setup: out[0] (host) = status (1: a non-finite observation, 2: a non-finite edge weight, 4: an edge id
- *   outside [0, n)); when 0, the arc CSR, one component (root 0, its mean as value), no active edge.
+ *   outside [0, n)); when 0, the arc CSR, one component (root 0, its mean as value), no active edge, every vertex
+ *   weight 1 (libcp.cutpursuit, cutpursuit.cpp:91).
+ * spg_cp_node_weights (after spg_cp_setup; libcp.cutpursuit2, cutpursuit.cpp:107-128): copies node_weight [n]
+ *   (device) as the vertex weights; out[0] (host) = status (8: a negative or non-finite weight); when 0, the one
+ *   component's value = sum w x / sum w and weight = sum w (all weights 0: NaN value).  Every later stage weighs
+ *   its sums, centres, terminal capacities, merge gains and energy by them (CutPursuit_SPG.h).
  * spg_cp_members: members / offsets = the vertices grouped by component, ascending.
  * spg_cp_kmeans: labels = 0, then 2-means per unsaturated component of >= 2 vertices (members current).
  * spg_cp_centers: c0 / c1 of every unsaturated component; L2 saturates a component with an empty side.
@@ -857,6 +864,8 @@ int spg_cp_regions(int64_t n, int64_t n_edges, int dim, int64_t* offsets);
 int spg_cp_setup(const float* obs, const int64_t* source, const int64_t* target, const float* edge_weight,
                  int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t* out,
                  spg_stream_t stream);
+int spg_cp_node_weights(const float* node_weight, int64_t n, int64_t n_edges, int dim, void* workspace,
+                        int64_t workspace_bytes, int64_t* out, spg_stream_t stream);
 int spg_cp_members(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,
                    spg_stream_t stream);
 int spg_cp_kmeans(int64_t n, int64_t n_edges, int dim, void* workspace, int64_t workspace_bytes, int64_t n_comp,

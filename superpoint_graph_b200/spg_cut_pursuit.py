@@ -1,18 +1,22 @@
 """The l0 cut pursuit partition on the device: `libcp.cutpursuit` of both partition pipelines (ref:
 partition/cut-pursuit/src/cutpursuit.cpp:77-105; called at partition/partition.py:177 and
-supervized_partition/losses.py:82).
+supervized_partition/losses.py:82), and the node-weighted `libcp.cutpursuit2` (cutpursuit.cpp:107-128) that
+supervized_partition/graph_processing.py:163 uses to inpaint Semantic3D's labels.
 
     from superpoint_graph_b200.spg_cut_pursuit import cutpursuit, to_numpy
 
     components, in_component = cutpursuit(features, source, target, edge_weight, reg_strength)
     graph_sp = compute_sp_graph(xyz, d_max, in_component, components, labels, n_labels)
+    components, in_component = cutpursuit2(obs, source, target, edge_weight, node_weight, reg_strength)
 
 Same arguments as libcp (speed 4: 3 flow steps, 10 k-means restarts of 5 iterations, at most 15 iterations, a
 backward merge step, stopping ratio 0.05; every vertex weighs 1).  spatial = 0 is CutPursuit_L2, 1 is
 CutPursuit_SPG.  in_component is an int64 CUDA tensor and components a `Components` CSR value (len() and indexing);
 to_numpy gives libcp's types.  The k-means draws are Philox4x32-10 keyed by `seed`, so a partition is reproducible;
 the minimal-cut colouring, the component numbering and the merge selection are the reference's (DESIGN.md §4).
-The kernels are in csrc/cut_pursuit.cu.
+cutpursuit2 is CutPursuit_SPG with the caller's vertex weights, cutoff 0 and weight_decay 1; a vertex of weight 0
+holds no observation, and a component whose weights are all 0 has the value NaN and is never merged, as in the
+reference.  The kernels are in csrc/cut_pursuit.cu.
 """
 import math
 
@@ -22,12 +26,12 @@ import torch
 from . import _lib, ops
 from ._inputs import check_dtype, check_ints, device_of, on_device
 
-__all__ = ["Components", "cutpursuit", "to_numpy", "compute_partition"]
+__all__ = ["Components", "cutpursuit", "cutpursuit2", "to_numpy", "compute_partition"]
 
 FLOW_STEPS, MAX_ITE_MAIN, STOPPING_RATIO, CUTOFF_ROUNDS = 3, 15, 0.05, 50
 REGIONS = ("obs", "comp", "root", "sat", "label", "colour", "active", "value", "c0", "c1", "cs", "ct", "ecap",
            "members", "offsets", "words", "dwords", "partner", "res", "excess", "rt", "arc_off", "arc_dst", "arc_rev",
-           "arc_edge")
+           "arc_edge", "nw", "cw")
 
 
 class Components:
@@ -67,7 +71,7 @@ def unary_weights(weight_decay):
 class State:
     """The device state of one cut pursuit: the workspace and the stage calls on it (csrc/cut_pursuit.cu)."""
 
-    def __init__(self, obs, source, target, edge_weight):
+    def __init__(self, obs, source, target, edge_weight, node_weight=None):
         self.n, self.D = obs.shape
         self.E = source.numel()
         self.dev = obs.device
@@ -76,6 +80,9 @@ class State:
         self.dout = torch.zeros(4, dtype=torch.float64)
         self._call("spg_cp_setup", obs, source, target, edge_weight, *self._dims(), self.out)
         self.status = int(self.out[0])
+        if node_weight is not None and self.status == 0:
+            self._call("spg_cp_node_weights", node_weight, *self._dims(), self.out)
+            self.status = int(self.out[0])
         self.n_comp = 1
 
     def _dims(self):
@@ -189,8 +196,9 @@ class _Null:
         return False
 
 
-def prepare(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial=0, weight_decay=1.0):
-    """Host validation and the device state; see cutpursuit."""
+def prepare(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial=0, weight_decay=1.0, node_weight=None):
+    """Host validation and the device state; see cutpursuit and cutpursuit2 (node_weight: float32 [n], every vertex
+    weighs 1 when None)."""
     shape = tuple(obs.shape)
     if len(shape) != 2 or shape[0] < 1:
         raise ValueError("obs must be [n, D] with n >= 1 (got shape %s)" % (shape,))
@@ -213,19 +221,27 @@ def prepare(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial=0,
     if len(set(sizes)) != 1:
         raise ValueError("source, target and edge_weight must have one entry per edge (got %d, %d, %d)"
                          % tuple(sizes))
-    dev = device_of(obs, source, target, edge_weight)
+    if node_weight is not None:
+        check_dtype(node_weight, "node_weight", "float32")
+        m = node_weight.numel() if torch.is_tensor(node_weight) else np.asarray(node_weight).size
+        if m != n:
+            raise ValueError("node_weight must have one entry per vertex (got %d for %d vertices)" % (m, n))
+    dev = device_of(obs, source, target, edge_weight, node_weight)
     obs_t = on_device(obs, dev)
     w = on_device(edge_weight, dev).reshape(-1)
     src = on_device(source, dev, int64=True).reshape(-1)
     tgt = on_device(target, dev, int64=True).reshape(-1)
+    nw = None if node_weight is None else on_device(node_weight, dev).reshape(-1)
     with torch.cuda.device(dev):
-        state = State(obs_t, src, tgt, w)
+        state = State(obs_t, src, tgt, w, nw)
     if state.status & 4:
         raise IndexError("an edge id is outside [0, %d)" % n)
     if state.status & 1:
         raise ValueError("obs contains NaN or infinity")
     if state.status & 2:
         raise ValueError("edge_weight contains NaN or infinity")
+    if state.status & 8:
+        raise ValueError("node_weight contains a negative weight, NaN or infinity")
     return state
 
 
@@ -239,6 +255,21 @@ def cutpursuit(obs, source, target, edge_weight, reg_strength, cutoff=0, spatial
     state = prepare(obs, source, target, edge_weight, reg_strength, cutoff, spatial, weight_decay)
     with torch.cuda.device(state.dev):
         run(state, reg_strength, cutoff, spatial, weight_decay, seed)
+        return state.output()
+
+
+def cutpursuit2(obs, source, target, edge_weight, node_weight, reg_strength, seed=0):
+    """(components, in_component) of libcp.cutpursuit2 (ref: cutpursuit.cpp:107-128): CutPursuit_SPG with the vertex
+    weights node_weight (float32 [n], >= 0), cutoff 0, weight_decay 1 (unary weights 1), speed 4.  A vertex of weight
+    0 holds no observation: it takes the component its edges lead it to, and a component whose weights are all 0 keeps
+    the value NaN and is never merged (DESIGN.md §4).
+
+    TypeError: obs, edge_weight or node_weight not float32, non-integer ids.  ValueError: shapes, D outside [1, 32],
+    non-finite observations or edge weights, a negative or non-finite node weight.  IndexError: an edge id outside
+    [0, n)."""
+    state = prepare(obs, source, target, edge_weight, reg_strength, 0, 1, 1.0, node_weight=node_weight)
+    with torch.cuda.device(state.dev):
+        run(state, reg_strength, 0, 1, 1.0, seed)
         return state.output()
 
 

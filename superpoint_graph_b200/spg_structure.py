@@ -27,7 +27,7 @@ import torch
 
 from . import ops, spg_delaunay, spg_geometry
 from ._inputs import check_dtype, check_ints, device_of, n_points, on_device, simplices_on
-from .spg_cut_pursuit import Components
+from .spg_cut_pursuit import Components, cutpursuit2
 
 __all__ = ["compute_graph_nn_2", "connected_comp", "compute_structure", "inpainting_problem", "to_numpy",
            "as_read_structure"]
@@ -138,8 +138,8 @@ def _transitions(lab, graph_nn, mode=ops.ST_DIFFERENT):
 
 
 def inpainting_problem(labels, graph_nn):
-    """The node-weighted problem graph_processing.py:152-162 hands to libcp.cutpursuit2 for sema3d (cut pursuit
-    with node weights is not computed on the device): (hard_labels int64 [n], edg_source, edg_target int64 (the
+    """The node-weighted problem graph_processing.py:152-162 hands to libcp.cutpursuit2 for sema3d
+    (spg_cut_pursuit.cutpursuit2 solves it): (hard_labels int64 [n], edg_source, edg_target int64 (the
     non-transition edges, in edge order), edge_weight float32 ones, node_weight float32 (0 where the label row
     labels[:, 1:] is empty, else 1)).  The transitions keep :155's operator precedence,
     hard[s] != (hard[t] * (hard[s] != 0) * (hard[t] != 0))."""
@@ -176,7 +176,8 @@ def _plane(xyz, bounds, low):
     return float(coef[0]), float(coef[1]), float(np.float64(reg.estimator_.intercept_))
 
 
-def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True, simplices=None):
+def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True, simplices=None, inpaint=False,
+                      seed=0):
     """graph_processing.py:124-126 and :144-193 on the device: a dict of write_structure's arguments, xyz, rgb,
     graph_nn, target_local_geometry (int64 [n, k_nn_local]), is_transition (uint8), labels, objects (int64), geof
     (float32 [n, 4], column 3 doubled, or None), elevation (float32 [n]) and xyn (float32 [n, 2]).
@@ -188,9 +189,12 @@ def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True
       vkitti  labels: the [n, C] histogram; objects = connected_comp of the edges whose hard labels (first argmax)
               agree, is_transition = hard[s] != hard[t].
       sema3d  labels None: labels = objects = [0], is_transition = False (:136-138).  With labels the objects come
-              from libcp.cutpursuit2 on inpainting_problem(labels, graph_nn), which the device does not compute:
-              pass them as objects= (else NotImplementedError); is_transition follows :165.
-    Other datasets raise ValueError.  The reference's geof = 0 without compute_geof makes write_structure's len(geof)
+              from libcp.cutpursuit2 on inpainting_problem(labels, graph_nn) (:150-165): inpaint=True computes them
+              with spg_cut_pursuit.cutpursuit2 (lambda 0.01, k-means draws keyed by seed, so they equal libcp's
+              only up to those draws), or pass them as objects= (else NotImplementedError); is_transition =
+              objects[source] != objects[target] over every edge (:165).
+    inpaint=True anywhere else (another dataset, no labels, objects given) raises ValueError.  Other datasets raise
+    ValueError.  The reference's geof = 0 without compute_geof makes write_structure's len(geof)
     raise; here geof is None.  With plane_model the low points are fitted by sklearn's RANSACRegressor(random_state=0)
     on the host and elevation = float32(z - (x c0 + y c1 + b)) in fp64 on the device."""
     if dataset not in _DATASETS:
@@ -199,9 +203,12 @@ def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True
     voronoi, want_geof, plane_model = (_field(args, "use_voronoi"), _field(args, "compute_geof"),
                                        _field(args, "plane_model"))
     n = n_points(np.shape(xyz))
-    if dataset == "sema3d" and labels is not None and objects is None:
-        raise NotImplementedError("sema3d with labels needs libcp.cutpursuit2 (node-weighted cut pursuit), which is "
-                                  "not computed on the device: pass its objects as objects=, see inpainting_problem")
+    if inpaint and (dataset != "sema3d" or labels is None or objects is not None):
+        raise ValueError("inpaint=True makes the objects of sema3d from its labels: it needs dataset 'sema3d', labels "
+                         "and no objects")
+    if dataset == "sema3d" and labels is not None and objects is None and not inpaint:
+        raise NotImplementedError("sema3d with labels needs the objects of libcp.cutpursuit2 (node-weighted cut "
+                                  "pursuit): pass inpaint=True to compute them on the device, or pass them as objects=")
     if dataset == "s3dis" and objects is None:
         raise ValueError("s3dis needs objects")
     if dataset == "vkitti" and labels is None:
@@ -224,8 +231,12 @@ def compute_structure(args, dataset, xyz, rgb, labels, objects=None, pruned=True
         else:
             check_ints(labels, "labels")
             lab = on_device(labels, dev, int64=True)
-            obj = _per_vertex(objects, "objects", n, dev)
+            obj = None if inpaint else _per_vertex(objects, "objects", n, dev)
         graph_nn, target2 = compute_graph_nn_2(x, k_adj, k_local, voronoi=voronoi, simplices=simplices)
+        if inpaint:
+            hard, s, t, edge_weight, node_weight = inpainting_problem(lab, graph_nn)
+            obj = cutpursuit2(hard.to(torch.float32).reshape(n, 1), s, t, edge_weight, node_weight, 0.01,
+                              seed=seed)[1]
         if dataset == "vkitti":
             hard = ops.st_argmax(lab, 0, 0)[0]
             is_tr = _transitions(hard, graph_nn)
