@@ -1010,6 +1010,48 @@ int spg_batch_edges(const int32_t* src, const int32_t* tgt, int64_t n_edges, con
                     float* feats_out, int64_t* targets_out, void* workspace, int64_t workspace_bytes,
                     spg_stream_t stream);
 
+/* ---------------------------------------------------------------- the batch's draws on the device
+ * The random choices of loader (ref: learning/spg.py:117 random.sample, :135-137 random.shuffle, :209-214 the
+ * resample, :240-257 augment_cloud) with the reference's distributions, drawn from Philox4x32-10 keyed by `seed`.
+ * Counter layout: the 64-bit draw k of stream (a, b, purpose) is Philox(c0 = k >> 1, c1 = a, c2 = b, c3 = purpose)
+ * words (2(k & 1), 2(k & 1) + 1) as (low, high); purposes 1 permutation, 2 centres, 3 resample, 4 augmentation,
+ * 5 jitter.  Graph draws: (a, b) = (0, graph_pos), draw v for vertex (new id) v.  Training clouds: (a, b) =
+ * (superpoint id, graph_pos); resample draw j for output point j, augmentation draws 0 scale, 1 angle, 2 and 3 the
+ * mirrors, jitter element j F + f draws 2k and 2k + 1.  Evaluation clouds: (a, b) = the low and high words of
+ * id + test_seed_offset, purpose 3 | 0x100.  u53(x) = (x >> 11) 2^-53; an index below n is the high word of x n.
+ *
+ * batch_draw: perm [n] (permute) = the rank of each vertex in a stable sort of its permutation key (a uniform
+ * permutation; perm[i] = new id of vertex i), centres [n_centres] = the new ids of the n_centres smallest centre
+ * keys (a uniform subset independent of perm).  Workspace from spg_batch_draw_workspace.
+ * ref: learning/spg.py:117,135-137                                                                          */
+int spg_batch_draw_workspace(int64_t n_ver, int64_t* bytes);
+int spg_batch_draw(int64_t n_ver, int64_t seed, int64_t graph_pos, int permute, int64_t n_centres, int32_t* perm,
+                   int32_t* centres, void* workspace, int64_t workspace_bytes, spg_stream_t stream);
+/* batch_cloud_flags: one graph's slice [n_ver] of the batch's cloud table, from batch_select's out `selected`.
+ * Position i < selected[0] holds kept vertex id = selected[2 + i]: count = sp_count[id] (-1 for an id the store
+ * lacks, and for id >= n_ids), first_row = sp_first_row[id], flags = -2 missing, -1 count < minpts, else 0;
+ * valid = (selected[1] > 0 and flags == 0); key = graph_pos << 32 | id.  Other positions: flags -1, valid 0.
+ * batch_clouds: the stable compaction of the valid positions of the whole batch into start_out / count_out /
+ * key_out (the first sum(valid) entries).  Workspace from spg_batch_clouds_workspace.
+ * ref: learning/spg.py:146-152 (ptn_minpts), s3dis_dataset.py:151-158 (one dataset per superpoint)          */
+int spg_batch_cloud_flags(const int32_t* selected, int64_t n_ver, int64_t graph_pos, const int64_t* sp_first_row,
+                          const int32_t* sp_count, int64_t n_ids, int64_t minpts, int32_t* flags, int32_t* valid,
+                          int64_t* first_row, int32_t* count, int64_t* key, spg_stream_t stream);
+int spg_batch_clouds_workspace(int64_t n, int64_t* bytes);
+int spg_batch_clouds(const int32_t* valid, const int64_t* first_row, const int32_t* count, const int64_t* key,
+                     int64_t n, void* workspace, int64_t workspace_bytes, int64_t* start_out, int32_t* count_out,
+                     int64_t* key_out, spg_stream_t stream);
+/* batch_cloud_draw: the inputs of spg_cloud_build for n_clouds clouds of key / count (batch_clouds' outputs).
+ * sample_idx [n, L]: identity when count == L, the original points first when count < L, else uniform in
+ * [0, count).  xform [n, 9] (NULL: none; evaluation passes NULL): s = 1/scale + (scale - 1/scale) u when
+ * scale > 1, the rotation about z by 2 pi u when rotate == 1, each mirror when u < mirror_prob / 2, composed in
+ * float64 in augment_matrix's order.  jitter [n, L, F] (NULL: none): float32(clip(0.01 g, +-0.05)) with g the
+ * float64 Box-Muller normal of (1 - u53, u53).  train == 0 keys the resample by id + test_seed_offset.
+ * ref: learning/spg.py:207-214,240-257                                                                     */
+int spg_batch_cloud_draw(const int64_t* key, const int32_t* count, int64_t n_clouds, int n_points, int n_attribs,
+                         int64_t seed, int train, int64_t test_seed_offset, double scale, int rotate,
+                         double mirror_prob, int32_t* sample_idx, double* xform, float* jitter, spg_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -119,6 +119,10 @@ enum KernelId {
     K_ST_POINTS,
     K_SB_SELECT,
     K_SB_EDGES,
+    K_SB_DRAW,
+    K_SB_PERM,
+    K_SB_FLAGS,
+    K_SB_CLOUD_DRAW,
     K_COUNT
 };
 

@@ -41,6 +41,7 @@ static const char* kKernelNames[K_COUNT] = {
     "dt_check",          "dt_commit",          "dt_relocate",         "dt_output",
     "st_vor",            "st_cc",              "st_labels",           "st_select",
     "st_points",         "sb_select",          "sb_edges",
+    "sb_draw",           "sb_perm",            "sb_flags",            "sb_cloud_draw",
 };
 
 struct Record {

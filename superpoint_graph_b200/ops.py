@@ -1752,14 +1752,18 @@ def st_points(xyz, bounds, plane=None, elevation=None, xyn=None, low=None, geof=
 
 # ------------------------------------------------------------- superpoint graph batch builder
 
-def batch_select(src, tgt, adjacency, sizes, perm, centres, order, minpts, cut):
+def batch_select(src, tgt, adjacency, sizes, perm, centres, order, minpts, cut, out=None):
     """Sub-graph selection of one resident graph (see spg_batch_select).  adjacency: the spg_graph_build views
     (EccGraph.to(device)) of its target-sorted edges.  Returns (new_index int32 [n], edge_pos int32 [E + 1],
-    out int32 [2 + n] = kept vertices, kept edges, kept original ids)."""
-    _need_cuda(src, tgt, sizes, perm, centres)
+    out int32 [2 + n] = kept vertices, kept edges, kept original ids); `out` may be given (a contiguous int32
+    [2 + n] slice of a larger buffer)."""
+    _need_cuda(src, tgt, sizes, perm, centres, out)
     n, E = sizes.numel(), src.numel()
     i32 = dict(dtype=torch.int32, device=sizes.device)
-    new_index, edge_pos, out = torch.empty(n, **i32), torch.empty(E + 1, **i32), torch.empty(2 + n, **i32)
+    new_index, edge_pos = torch.empty(n, **i32), torch.empty(E + 1, **i32)
+    if out is None:
+        out = torch.empty(2 + n, **i32)
+    assert out.dtype == torch.int32 and out.is_contiguous() and out.numel() == 2 + n
     ws = _workspace("spg_batch_select_workspace", sizes.device, n, E)
     _lib.call("spg_batch_select", src, tgt, n, E, adjacency["tgt_rowptr"], adjacency["idxn"],
               adjacency["src_rowptr"], adjacency["src_perm"], adjacency["edge_tgt"], sizes, perm, centres,
@@ -1778,3 +1782,64 @@ def batch_edges(src, tgt, new_index, edge_pos, kept, n_kept, n_kept_edges, verte
     _lib.call("spg_batch_edges", src, tgt, src.numel(), new_index, edge_pos, kept, int(n_kept), int(n_kept_edges),
               int(vertex_offset), edge_feats, edge_feats.shape[1], targets, targets.shape[1], idxn_out, tgt_out,
               degs_out, feats_out, targets_out, ws, ws.numel(), _lib.current_stream())
+
+
+def _seed64(seed):
+    """A seed as the int64 with the same 64 bits (the C-ABI takes the key as int64_t)."""
+    s = int(seed) & 0xFFFFFFFFFFFFFFFF
+    return s - (1 << 64) if s >= (1 << 63) else s
+
+
+def batch_draw(n, seed, graph_pos, permute, n_centres, device):
+    """(perm int32 [n] or None, centres int32 [n_centres] or None) on the device: the graph draws of position
+    `graph_pos` of a batch under `seed` (see spg_batch_draw)."""
+    i32 = dict(dtype=torch.int32, device=device)
+    perm = torch.empty(n, **i32) if permute else None
+    centres = torch.empty(n_centres, **i32) if n_centres > 0 else None
+    if perm is None and centres is None:
+        return None, None
+    ws = _workspace("spg_batch_draw_workspace", device, n)
+    _lib.call("spg_batch_draw", int(n), _seed64(seed), int(graph_pos), int(bool(permute)), int(n_centres), perm,
+              centres, ws, ws.numel(), _lib.current_stream())
+    return perm, centres
+
+
+def batch_cloud_flags(selected, graph_pos, sp_index, minpts, flags, valid, first_row, count, key):
+    """One graph's slice of the batch's cloud table from batch_select's `selected` (see spg_batch_cloud_flags);
+    sp_index = (first row int64 [ids], count int32 [ids]) of the file in the superpoint store, or None."""
+    _need_cuda(selected, flags, valid, first_row, count, key)
+    rows, counts = sp_index if sp_index is not None else (None, None)
+    n_ids = 0 if counts is None else counts.numel()
+    _lib.call("spg_batch_cloud_flags", selected, flags.numel(), int(graph_pos), rows, counts, int(n_ids), int(minpts),
+              flags, valid, first_row, count, key, _lib.current_stream())
+
+
+def batch_clouds(valid, first_row, count, key):
+    """(start int64 [n], count int32 [n], key int64 [n]) whose first sum(valid) entries are the valid positions'
+    values in order (see spg_batch_clouds)."""
+    _need_cuda(valid, first_row, count, key)
+    n, dev = valid.numel(), valid.device
+    start_out, key_out = torch.empty(n, dtype=torch.int64, device=dev), torch.empty(n, dtype=torch.int64, device=dev)
+    count_out = torch.empty(n, dtype=torch.int32, device=dev)
+    ws = _workspace("spg_batch_clouds_workspace", dev, n)
+    _lib.call("spg_batch_clouds", valid, first_row, count, key, n, ws, ws.numel(), start_out, count_out, key_out,
+              _lib.current_stream())
+    return start_out, count_out, key_out
+
+
+def batch_cloud_draw(key, count, n_clouds, n_points, n_attribs, seed, train, test_seed_offset=0, scale=0.0, rotate=0,
+                     mirror_prob=0.0, jitter=False):
+    """(sample_idx int32 [n, L], xform float64 [n, 9] or None, jitter float32 [n, L, F] or None) on the device: the
+    cloud draws of the first n_clouds entries of key / count (see spg_batch_cloud_draw).  Evaluation (train False)
+    draws neither matrices nor jitter."""
+    _need_cuda(key, count)
+    assert key.dtype == torch.int64 and count.dtype == torch.int32
+    dev = key.device
+    idx = torch.empty((n_clouds, n_points), dtype=torch.int32, device=dev)
+    xform = torch.empty((n_clouds, 9), dtype=torch.float64, device=dev) if train else None
+    noise = (torch.empty((n_clouds, n_points, n_attribs), dtype=torch.float32, device=dev)
+             if train and jitter else None)
+    _lib.call("spg_batch_cloud_draw", key, count, int(n_clouds), int(n_points), int(n_attribs), _seed64(seed),
+              int(bool(train)), int(test_seed_offset), float(scale), int(rotate), float(mirror_prob), idx, xform,
+              noise, _lib.current_stream())
+    return idx, xform, noise

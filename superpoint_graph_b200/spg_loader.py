@@ -47,6 +47,7 @@ class SuperpointStore(object):
         self._chunks, self._index, self._rows = [], {}, 0
         self.points = None
         self.n_columns = None
+        self._dense, self._columns = {}, {}
 
     def add(self, fname, superpoints):
         for sp_id, P in superpoints.items():
@@ -73,6 +74,18 @@ class SuperpointStore(object):
             r += P.shape[0]
         self.points = torch.from_numpy(host).to(device)
         self._chunks = []
+        # per file, dense by superpoint id: first row (int64) and count (int32, -1 for an id the store lacks)
+        per_file = {}
+        for (fname, sp_id), (row, n) in self._index.items():
+            if sp_id >= 0:
+                per_file.setdefault(fname, []).append((sp_id, row, n))
+        self._dense = {}
+        for fname, entries in per_file.items():
+            ids, rows, counts = (np.array(c, dtype=np.int64) for c in zip(*entries))
+            first = np.zeros(int(ids.max()) + 1, np.int64)
+            count = -np.ones(int(ids.max()) + 1, np.int32)
+            first[ids], count[ids] = rows, counts
+            self._dense[fname] = (torch.from_numpy(first).to(device), torch.from_numpy(count).to(device))
         return self
 
     def count(self, fname, sp_id):
@@ -80,6 +93,23 @@ class SuperpointStore(object):
 
     def start(self, fname, sp_id):
         return self._index[(fname, int(sp_id))][0]
+
+    def device_index(self, fname):
+        """(first row int64 [ids], count int32 [ids]) on the device, indexed by superpoint id (count -1: not in the
+        store), or None for a file without superpoints."""
+        return self._dense.get(fname)
+
+    def device_columns(self, cols):
+        """The source columns `cols` as a device int32 tensor, kept per column list; written element by element
+        from the host's integers, so no host buffer is copied and the stream is not synchronised."""
+        cols = tuple(cols)
+        t = self._columns.get(cols)
+        if t is None:
+            t = torch.empty(len(cols), dtype=torch.int32, device=self.points.device)
+            for f, c in enumerate(cols):
+                t[f:f + 1].fill_(c)
+            self._columns[cols] = t
+        return t
 
 
 def sample_indices(n, npts, rs):
@@ -244,7 +274,7 @@ def graph_draws(n, train, args):
     return perm, centres, max(hc, 0)
 
 
-def load_batch(gstore, cstore, names, train, args, test_seed_offset=0):
+def load_batch(gstore, cstore, names, train, args, test_seed_offset=0, device_rng=False, seed=0):
     """`loader(entry, train, args, db_path, test_seed_offset)` for every name, then `eccpc_collate`
     (ref: learning/spg.py:130-193).  Returns (targets, GIs, (clouds_meta, clouds_flag, clouds, clouds_global))
     with targets int64 [N, 2 + C], clouds and clouds_global on the device, GIs = [GraphConvInfo] whose idxn,
@@ -254,9 +284,17 @@ def load_batch(gstore, cstore, names, train, args, test_seed_offset=0):
     and kept ids (none when the whole graph is kept; one copy of the whole [2 + n] word array, so one
     synchronisation, where reading the count first would take two), then load_superpoints' cloud draws for graphs with edges.
     Graphs without edges are dropped; the collate's exceptions are the reference's (RuntimeError when no graph
-    has an edge, TypeError when the first has none or a graph with edges has no cloud)."""
-    from .spg_ecc import GraphConvInfo
+    has an edge, TypeError when the first has none or a graph with edges has no cloud).
 
+    device_rng=True draws every random choice of the batch on the device instead (Philox4x32-10 keyed by `seed`;
+    the reference's distributions, not its streams; Python's `random` and numpy's global state are not touched) and
+    builds the batch with one synchronisation whatever the number of graphs: every graph's draws, selection and
+    cloud table are enqueued first, then one read-back of the counts, kept ids and flags sizes the rest.  Training
+    streams are keyed by (seed, position in `names`, superpoint or vertex), evaluation clouds by (seed,
+    id + test_seed_offset); see include/spg_b200.h spg_batch_draw for the counter layout.  KeyError for a kept
+    superpoint of a graph with edges that the store lacks, as store.count raises on the host path."""
+    if device_rng:
+        return _load_batch_device(gstore, cstore, names, train, args, test_seed_offset, seed)
     dev = gstore.device
     picks = []
     for name in names:
@@ -276,12 +314,27 @@ def load_batch(gstore, cstore, names, train, args, test_seed_offset=0):
             ids, kept_dev = host[2:2 + n_kept].tolist(), out[2:2 + n_kept]
         clouds = load_superpoints(cstore, name, ids, args, train, test_seed_offset) if n_edges else None
         picks.append((f, new_index, edge_pos, kept_dev, n_kept, n_edges, ids, clouds))
+    kept, targets, gi = _collate(dev, picks, [p[7][1].shape[0] if p[5] else 0 for p in picks])
+    clouds_meta = ["{}.{:d}".format(p[0]["name"], v) for p in kept for v in p[6]]
+    clouds_flag = torch.from_numpy(np.concatenate([p[7][0] for p in kept]))
+    clouds = torch.cat([p[7][1] for p in kept], 0)
+    clouds_global = torch.cat([p[7][2] for p in kept], 0)
+    return targets, [gi], (clouds_meta, clouds_flag, clouds, clouds_global)
+
+
+def _collate(dev, picks, n_clouds):
+    """eccpc_collate's graph part (ref: learning/spg.py:178-193).  picks: per graph (file, new_index, edge_pos,
+    kept ids on the device, n_kept, n_edges, kept ids, clouds); new_index None: the whole graph is kept.  n_clouds:
+    per graph, its clouds of at least ptn_minpts points.  Raises the collate's exceptions; returns (the picks of the
+    graphs with edges, targets, GraphConvInfo)."""
+    from .spg_ecc import GraphConvInfo
+
     kept = [p for p in picks if p[5]]
     if not kept:
         raise RuntimeError("torch.cat(): expected a non-empty list of Tensors")
     if not picks[0][5]:
         raise TypeError("object of type 'NoneType' has no len()")
-    if any(p[7][1].shape[0] == 0 for p in kept):
+    if any(c == 0 for p, c in zip(picks, n_clouds) if p[5]):
         raise TypeError("expected np.ndarray (got list)")
     feats_w = {p[0]["feats"].shape[1] for p in kept}
     cols = {p[0]["targets"].shape[1] for p in kept}
@@ -302,9 +355,58 @@ def load_batch(gstore, cstore, names, train, args, test_seed_offset=0):
                         f["targets"], edge_index[0, eo:eo + n_edges], edge_index[1, eo:eo + n_edges],
                         degs[vo:vo + n_kept], edgefeats[eo:eo + n_edges], targets[vo:vo + n_kept])
         vo, eo = vo + n_kept, eo + n_edges
-    gi = GraphConvInfo.from_device_arrays(edge_index, degs, edgefeats)
-    clouds_meta = ["{}.{:d}".format(p[0]["name"], v) for p in kept for v in p[6]]
-    clouds_flag = torch.from_numpy(np.concatenate([p[7][0] for p in kept]))
-    clouds = torch.cat([p[7][1] for p in kept], 0)
-    clouds_global = torch.cat([p[7][2] for p in kept], 0)
+    return kept, targets, GraphConvInfo.from_device_arrays(edge_index, degs, edgefeats)
+
+
+def _load_batch_device(gstore, cstore, names, train, args, test_seed_offset, seed):
+    """load_batch(device_rng=True): graph draws, selection and cloud table of every graph, one read-back, then the
+    cloud draws, the clouds and the collated edges."""
+    if cstore.points is None:
+        raise RuntimeError("SuperpointStore.finalize(device) has not been called")
+    dev = gstore.device
+    files = [gstore.file(name) for name in names]
+    hc, nn = (int(args.spg_augm_hardcutoff), int(args.spg_augm_nneigh)) if train else (0, 0)
+    order, minpts = int(args.spg_augm_order) if train else 0, int(args.ptn_minpts)
+    n_all = sum(f["n"] for f in files)
+    fo = 2 * len(files) + n_all
+    # read back at once: every graph's [2 + n] selection words, then every graph's [n] clouds_flag
+    words = torch.empty(fo + n_all, dtype=torch.int32, device=dev)
+    valid, count = torch.empty(n_all, dtype=torch.int32, device=dev), torch.empty(n_all, dtype=torch.int32, device=dev)
+    first_row, key = torch.empty(n_all, dtype=torch.int64, device=dev), torch.empty(n_all, dtype=torch.int64, device=dev)
+    graphs, o, v = [], 0, 0
+    for b, f in enumerate(files):
+        n = f["n"]
+        perm, centres = ops.batch_draw(n, seed, b, 0 < hc < n, nn if 0 < nn < n else 0, dev)
+        out = words[o:o + 2 + n]
+        new_index, edge_pos, _ = ops.batch_select(f["src"], f["tgt"], f["adjacency"], f["s"], perm, centres, order,
+                                                  minpts, max(hc, 0), out=out)
+        sl = slice(v, v + n)
+        ops.batch_cloud_flags(out, b, cstore.device_index(f["name"]), minpts, words[fo + v:fo + v + n], valid[sl],
+                              first_row[sl], count[sl], key[sl])
+        graphs.append((f, new_index, edge_pos, out, o, v))
+        o, v = o + 2 + n, v + n
+    start, n_points, cloud_key = ops.batch_clouds(valid, first_row, count, key)
+    host = words.cpu().numpy()
+    picks = []
+    for f, new_index, edge_pos, out, o, v in graphs:
+        n_kept, n_edges = int(host[o]), int(host[o + 1])
+        ids, flags = host[o + 2:o + 2 + n_kept], host[fo + v:fo + v + n_kept]
+        if n_edges and (flags == -2).any():
+            raise KeyError((f["name"], int(ids[np.argmax(flags == -2)])))
+        picks.append((f, new_index, edge_pos, out[2:2 + n_kept], n_kept, n_edges, ids, flags))
+    n_clouds = [int((p[7] == 0).sum()) for p in picks]
+    kept, targets, gi = _collate(dev, picks, n_clouds)
+    nv, L = sum(c for p, c in zip(picks, n_clouds) if p[5]), int(args.ptn_npts)
+    cols = attrib_columns(args.pc_attribs, cstore.n_columns)
+    clouds = torch.empty((nv, len(cols), L), dtype=torch.float32, device=dev)
+    clouds_global = torch.empty((nv,), dtype=torch.float32, device=dev)
+    if nv:
+        aug = (float(args.pc_augm_scale), int(args.pc_augm_rot), float(args.pc_augm_mirror_prob),
+               bool(getattr(args, "pc_augm_jitter", 0))) if train else (0.0, 0, 0.0, False)
+        idx, mats, noise = ops.batch_cloud_draw(cloud_key, n_points, nv, L, len(cols), seed, train, test_seed_offset,
+                                                *aug)
+        ops.cloud_build(cstore.points, start, n_points, idx, cstore.device_columns(cols), L,
+                        bool(args.pc_xyznormalize), mats, noise, 0.0, 0.05, 0, clouds, clouds_global)
+    clouds_meta = [p[0]["name"] + "." + str(v) for p in kept for v in p[6].tolist()]
+    clouds_flag = torch.from_numpy(np.concatenate([p[7] for p in kept]).astype(np.int64))
     return targets, [gi], (clouds_meta, clouds_flag, clouds, clouds_global)

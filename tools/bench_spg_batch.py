@@ -15,6 +15,12 @@ cloud_build, uploads, read-backs, collation copies).  With
 SPG_REFERENCE set to a reference checkout, the reference's `loader` + `eccpc_collate` run on the host cores over
 the compat igraph stand-in (compat/igraph.py: real igraph is not required) on the same graphs; without it that arm
 is reported as "not measured".
+
+Each workload also runs the `device_rng=True` arm (`seed` = the run's index), alternated run by run with the host
+arm in the same timed loop.  Per arm: the end-to-end median, the profiled device time, the synchronising operations
+torch reports under `torch.cuda.set_sync_debug_mode("warn")` in one call, and the time the arm spends formatting
+`clouds_meta` from the kept ids (timed apart on the ids of one batch).  The host arm keeps the keys above; the
+device arm's are under "device_rng".
 """
 import argparse
 import json
@@ -24,6 +30,7 @@ import subprocess
 import sys
 import time
 import types
+import warnings
 from types import SimpleNamespace
 
 import numpy as np
@@ -57,30 +64,69 @@ def clouds_for(rng, counts, cap):
     return {i: rng.standard_normal((int(min(c, cap)), 14)).astype(np.float32) for i, c in enumerate(counts)}
 
 
+def call(gs, cs, names, train, args, r, device_rng):
+    if device_rng:
+        return spg_loader.load_batch(gs, cs, names, train, args, device_rng=True, seed=r)
+    random.seed(r)
+    np.random.seed(r)
+    return spg_loader.load_batch(gs, cs, names, train, args)
+
+
 def time_product(gs, cs, names, train, args, reps):
-    ends = []
+    """End-to-end medians (host arm, device_rng arm), the arms alternated run by run."""
+    ends = {False: [], True: []}
     for r in range(reps + 3):
-        random.seed(r)
-        np.random.seed(r)
-        torch.cuda.synchronize()
+        for device_rng in (False, True):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            call(gs, cs, names, train, args, r, device_rng)
+            torch.cuda.synchronize()
+            if r >= 3:
+                ends[device_rng].append(1e3 * (time.perf_counter() - t0))
+    return float(np.median(ends[False])), float(np.median(ends[True]))
+
+
+def sync_count(gs, cs, names, train, args, device_rng):
+    """Synchronising operations torch reports in one call (after one unreported call)."""
+    call(gs, cs, names, train, args, 0, device_rng)
+    torch.cuda.synchronize()
+    with warnings.catch_warnings(record=True) as caught:
+        warnings.simplefilter("always")
+        torch.cuda.set_sync_debug_mode("warn")
+        try:
+            call(gs, cs, names, train, args, 1, device_rng)
+        finally:
+            torch.cuda.set_sync_debug_mode("default")
+    return sum("synchronizing" in str(w.message) for w in caught)
+
+
+def meta_time(gs, cs, names, train, args, device_rng, reps=5):
+    """ms to format one batch's clouds_meta from its kept ids, as the arm's load_batch does."""
+    meta = call(gs, cs, names, train, args, 0, device_rng)[2][0]
+    ids = {}
+    for m in meta:
+        nm, v = m.rsplit(".", 1)
+        ids.setdefault(nm, []).append(int(v))
+    kept = [(nm, np.array(v, np.int32) if device_rng else v) for nm, v in ids.items()]
+    out = []
+    for _ in range(reps):
         t0 = time.perf_counter()
-        spg_loader.load_batch(gs, cs, names, train, args)
-        torch.cuda.synchronize()
-        if r >= 3:
-            ends.append(1e3 * (time.perf_counter() - t0))
-    return float(np.median(ends))
+        if device_rng:
+            [nm + "." + str(v) for nm, vv in kept for v in vv.tolist()]
+        else:
+            ["{}.{:d}".format(nm, v) for nm, vv in kept for v in vv]
+        out.append(1e3 * (time.perf_counter() - t0))
+    return float(np.median(out))
 
 
-def device_time(gs, cs, names, train, args, reps):
+def device_time(gs, cs, names, train, args, reps, device_rng=False):
     """(all device ms, graph-builder kernel ms) per call, means over `reps` profiled calls."""
     from torch.profiler import ProfilerActivity, profile
 
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for r in range(reps):
-            random.seed(r)
-            np.random.seed(r)
-            spg_loader.load_batch(gs, cs, names, train, args)
+            call(gs, cs, names, train, args, r, device_rng)
         torch.cuda.synchronize()
     total = graph = 0.0
     for ev in prof.key_averages():
@@ -157,13 +203,20 @@ def main():
             names.append(nm)
         gs.finalize("cuda")
         cs.finalize("cuda")
-        end = time_product(gs, cs, names, train, args, opt.reps)
+        end, end_rng = time_product(gs, cs, names, train, args, opt.reps)
         dev_all, dev_graph = device_time(gs, cs, names, train, args, opt.reps)
+        rng_all, rng_graph = device_time(gs, cs, names, train, args, opt.reps, device_rng=True)
         result[tag] = {"vertices": sizes, "edges": [int(graphs[nm][2].shape[0]) for nm in names],
                        "load_batch_ms": round(end, 3), "device_ms": round(dev_all, 4),
                        "device_graph_kernels_ms": round(dev_graph, 4),
                        "reference_host_compat_igraph_ms": time_reference(graphs, clouds, names, train, args,
-                                                                          opt.reps)}
+                                                                          opt.reps),
+                       "syncs": sync_count(gs, cs, names, train, args, False),
+                       "clouds_meta_ms": round(meta_time(gs, cs, names, train, args, False), 3),
+                       "device_rng": {"load_batch_ms": round(end_rng, 3), "device_ms": round(rng_all, 4),
+                                      "device_graph_kernels_ms": round(rng_graph, 4),
+                                      "syncs": sync_count(gs, cs, names, train, args, True),
+                                      "clouds_meta_ms": round(meta_time(gs, cs, names, train, args, True), 3)}}
         print(json.dumps({tag: result[tag]}), file=sys.stderr, flush=True)
     print(json.dumps(result))
 
